@@ -4,18 +4,23 @@ lighting + HDR post chain on a 3840x2160 synthetic G-buffer with 4096 lights (BA
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path (torchrun for N > 1)
   python bench.py --impl reference --gpus N --steps K ...  # the reference's algorithm on the host cores
-                                                           # (CPU oracle; the reference has no CPU path
-                                                           #  and no Vulkan device exists here)
-Prints ONE JSON line on rank 0.  A "step" is one frame.
+                                                           # (CPU oracle; the reference has no CPU path)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed frame's output
+
+Prints ONE JSON line on rank 0.  A "step" is one frame.  Nothing is written into the source tree:
+the natively rebuilt oracle of the CPU baseline is compiled into a temporary directory.
 """
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import math
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -53,7 +58,7 @@ def algorithmic_bytes(w, h, aa, bloom=True):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -110,34 +115,24 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
-
-
-def ncu_traffic():
-    """dram bytes per launch of the lighting kernel from the committed ncu capture, if any."""
-    p = os.path.join(ROOT, "profiles", "lighting_traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get("dram_bytes_per_launch")
-        except Exception:
-            return None
-    return None
+    return 3350.0, "the H100 SXM data sheet (HBM3), not a measurement"
 
 
 # ------------------------------------------------------------------------------------------------
 def _native_oracle():
-    """The oracle rebuilt for THIS machine's cores (-O3 -march=native, BASELINE.md section 4) into
-    oracle/_build/native/: the in-tree liboracle.so is a portable -O2 build because it travels from the
-    build container to the GPU box.  Same sources, same -ffp-contract=off arithmetic contract."""
-    import subprocess
+    """The oracle rebuilt for THIS machine's cores (-O3 -march=native, BASELINE.md section 4) in a
+    temporary directory (the source tree may be read-only): the in-tree liboracle.so is a portable -O2
+    build because it may be built on another machine.  Same sources, same -ffp-contract=off arithmetic
+    contract."""
     from oracle import pyoracle as oracle
 
     src_dir = os.path.dirname(os.path.abspath(oracle.__file__))
-    out_dir = os.path.join(src_dir, "_build", "native")
-    out = os.path.join(out_dir, "liboracle.so")
     srcs = [os.path.join(src_dir, f) for f in ("oracle_host.c", "oracle_cluster.c", "oracle_lighting.c", "oracle_post.c", "oracle_smaa.c")]
     try:
-        os.makedirs(out_dir, exist_ok=True)
+        # kept for the life of the process (oracle.lib() may reload from _LIB_PATH), removed at exit
+        out_dir = tempfile.mkdtemp(prefix="grb_oracle_")
+        atexit.register(shutil.rmtree, out_dir, True)
+        out = os.path.join(out_dir, "liboracle.so")
         subprocess.run(["gcc", "-O3", "-march=native", "-std=c11", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-fopenmp", "-shared", "-o", out,
                         *srcs, "-lm"], check=True, capture_output=True)
         oracle._LIB_PATH = out
@@ -226,6 +221,25 @@ def oracle_frame_time(w, h, n_lights, aa, steps, warmup, budget_s=150.0, bloom=T
                         f"per step: cluster build + pyramid tail in full, per-pixel passes on rows [0,{rows}) of {h} scaled x{h / rows:.2f}")
 
 
+DUMP_MAX_PIXELS = 1 << 21  # 32 MB of float32 RGBA (+ 16 MB of sample indices) stays under 64 MB
+
+
+def dump_outputs(out_dir, v, out, w, h):
+    """Write what a caller of the timed path receives for the last timed frame -- the R8G8B8A8 output
+    image -- as float32 channel codes 0..255: `output_rgba8.npy` (H, W, 4) when the frame has at most
+    DUMP_MAX_PIXELS pixels, else `output_rgba8_sample.npy` (N, 4) for a fixed seeded sample of
+    N = DUMP_MAX_PIXELS pixels, with their row-major indices in `output_sample_index.npy` (float64)."""
+    v.read_output(out)
+    rgba = out.numpy().view(np.uint8).reshape(h, w, 4)
+    os.makedirs(out_dir, exist_ok=True)
+    if w * h <= DUMP_MAX_PIXELS:
+        np.save(os.path.join(out_dir, "output_rgba8.npy"), rgba.astype(np.float32))
+        return
+    idx = np.sort(np.random.default_rng(0).choice(w * h, DUMP_MAX_PIXELS, replace=False))
+    np.save(os.path.join(out_dir, "output_rgba8_sample.npy"), rgba.reshape(-1, 4)[idx].astype(np.float32))
+    np.save(os.path.join(out_dir, "output_sample_index.npy"), idx.astype(np.float64))
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -235,20 +249,26 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="c3", choices=sorted(WORKLOADS))
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the output image of the last timed frame to DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
 
     w, h, n_lights, aa, desc = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.dump_outputs and (world > 1 or args.impl != "ours"):
+        ap.error("--dump-outputs needs --impl ours on one GPU (a rank reads back only its own rows)")
     bloom = args.workload not in NO_BLOOM
     lighting_b, chain_b, total_b = algorithmic_bytes(w, h, aa, bloom)
     config = {"workload": f"{args.workload}: {desc}", "width": w, "height": h, "lights": n_lights, "cluster_grid": "128x64x4096",
               "sharding": f"{world} row bands (8-row units): balanced by measured lighting time for the resident region, equal rows for the end-to-end region" if world > 1 else "none",
-              "l2": (f"per-frame inputs ({w * h * LIGHTING_BYTES_PER_PIXEL / 1e6:.0f} MB of G-buffer + HDR) exceed the 126 MB L2; no explicit flush"
-                     if w * h * LIGHTING_BYTES_PER_PIXEL > 126e6 else
-                     f"per-frame inputs ({w * h * LIGHTING_BYTES_PER_PIXEL / 1e6:.1f} MB) fit in the 126 MB L2 and are not flushed: not a headline configuration"),
+              "l2": (f"per-frame inputs ({w * h * LIGHTING_BYTES_PER_PIXEL / 1e6:.0f} MB of G-buffer + HDR) exceed the 50 MB L2; no explicit flush"
+                     if w * h * LIGHTING_BYTES_PER_PIXEL > 50e6 else
+                     f"per-frame inputs ({w * h * LIGHTING_BYTES_PER_PIXEL / 1e6:.1f} MB) fit in the 50 MB L2 and are not flushed: not a headline configuration"),
               "algorithmic_mb_per_frame": round(total_b / 1e6, 2)}
 
     if args.impl == "reference":
@@ -393,10 +413,9 @@ def main():
         time.sleep(0.3)
 
     # ---- timed region 1: device-resident inputs (value) ----
-    # A window is EXACTLY K steps between two events (barrier + synchronize on both sides, max over
-    # ranks).  K frames of this workload last a few milliseconds, which is too short to be a steady
-    # state on its own, so the window is repeated until at least 0.5 s of GPU time has been timed and
-    # `value` is the MEDIAN window (all windows are reported).
+    # One window of EXACTLY K = --steps frames between two events (barrier + synchronize on both
+    # sides, max over ranks).  Pass a K that makes the window last well over 0.1 s: a shorter window
+    # measures launch jitter as much as the frames.
     PREROLL = 4
 
     def resident_window():
@@ -419,16 +438,9 @@ def main():
         return max_over_ranks(e0.elapsed_time(e1)), host
 
     t_begin = time.time()
-    windows, hosts = [], []
-    while not windows or (sum(windows) < 500.0 and len(windows) < 400):
-        ms, host = resident_window()
-        windows.append(ms)
-        hosts.append(host)
-    ms_resident = float(np.median(windows))
-    host_ms = float(np.median(hosts))
-    srt = sorted(windows)
-    frame_stats = {"windows": len(windows), "steps_per_window": args.steps, "preroll_frames": PREROLL, "min": round(srt[0] / args.steps, 4), "p50": round(ms_resident / args.steps, 4),
-                   "max": round(srt[-1] / args.steps, 4)}
+    ms_resident, host_ms = resident_window()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, v, out, w, h)
 
     # ---- timed region 2: end to end through the host API.  Every step copies its G-buffer rows from
     # pinned host memory to the device and its result rows back; frames are pipelined two deep (the
@@ -493,15 +505,15 @@ def main():
         "gpu_launches": launches_per_frame * args.steps,
         "hbm_gbs_whole_frame": total_b / (ms_resident / args.steps * 1e-3) / 1e9 / 1.0,
         "roofline": {"kernel": "deferred_lighting_persistent_kernel (pass 'lighting')", "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": (achieved / peak) if achieved else None, "traffic": ncu_traffic(), "peak_source": f"of {peak_kind}",
+                     "frac": (achieved / peak) if achieved else None, "peak_source": f"from {peak_kind}",
                      "bytes_per_pixel": LIGHTING_BYTES_PER_PIXEL, "note": "ALU-bound at this light density: see DESIGN.md"},
         "pass_ms": {k: round(val, 4) for k, val in timings.items()},
         "host_record_ms_per_step": round(host_ms / args.steps, 4),
-        "ms_per_step_windows": frame_stats,
+        "preroll_frames": PREROLL,
     }
     # ---- the other single-GPU configurations of BASELINE.json (c2: 1080p / 1024 lights, c5: 4K TAA +
-    # FXAA with history): device-resident frames/s over one window of >= 0.25 s plus per-pass times,
-    # so that every configuration has a driver-run number.  Not part of `value`.
+    # FXAA with history): device-resident frames/s over one window of --steps frames plus per-pass
+    # times, so that every configuration has a number from the same run.  Not part of `value`.
     if rank == 0 and world == 1 and args.workload == "c3":
         line["other_configs"] = {}
         for name in ("c2", "c5"):
@@ -529,18 +541,15 @@ def main():
                     ov.render_frame(None)
                 ov.sync()
                 ov.collect_timings()
-                frames, total_ms = 0, 0.0
-                while total_ms < 250.0 and frames < 4000:
-                    a0, a1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    torch.cuda.synchronize()
-                    a0.record(stream)
-                    for _ in range(50):
-                        ov.render_frame(None)
-                    ov.join_streams()
-                    a1.record(stream)
-                    torch.cuda.synchronize()
-                    total_ms += a0.elapsed_time(a1)
-                    frames += 50
+                a0, a1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                a0.record(stream)
+                for _ in range(args.steps):
+                    ov.render_frame(None)
+                ov.join_streams()
+                a1.record(stream)
+                torch.cuda.synchronize()
+                frames, total_ms = args.steps, a0.elapsed_time(a1)
                 tm = {k: round(ms / max(c, 1), 4) for k, (ms, c) in ov.collect_timings().items()}
                 ov.close()
                 _, _, ob = algorithmic_bytes(ow, oh, oaa)

@@ -1,4 +1,4 @@
-"""granite_b200 -- B200-native (sm_100a) executor for Granite's clustered deferred lighting and
+"""granite_b200 -- H100-native (sm_90a) executor for Granite's clustered deferred lighting and
 HDR post chain.  The product is the C-ABI shared library libgranite_b200.so (include/granite_b200.h)
 plus the C++ host layer mirroring Granite's RenderGraph pass interface; this Python package is the
 thin ctypes/torch harness used by the tests and bench.py."""

@@ -1,4 +1,4 @@
-"""Builds libgranite_b200.so in-tree with nvcc for sm_100a (no torch extension machinery:
+"""Builds libgranite_b200.so in-tree with nvcc for sm_90a (no torch extension machinery:
 the product is a plain C-ABI shared library)."""
 from __future__ import annotations
 
@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgranite_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 # diagnostics only, e.g. GRB_EXTRA_NVCC_FLAGS=-DGRB_LIGHTING_DEBUG for tools/lighting_timeline.py
 COMMON += os.environ.get("GRB_EXTRA_NVCC_FLAGS", "").split()

@@ -1,5 +1,5 @@
 // grb_cluster.cu -- the bindless light clusterer (spot hull transform, per-light cull setup,
-// XY tile binning, per-slice Z range) as sm_100a kernels.  Compiled with -fmad=false: the
+// XY tile binning, per-slice Z range) as sm_90a kernels.  Compiled with -fmad=false: the
 // outputs are integers (bitmask words, index ranges) decided by fp32 comparisons, and the
 // contract with the reference/oracle is bit-exactness, so every fp32 op must round on its own.
 //

@@ -1,4 +1,4 @@
-// grb_common.cuh -- device-side helpers shared by the sm_100a kernels of libgranite_b200.
+// grb_common.cuh -- device-side helpers shared by the sm_90a kernels of libgranite_b200.
 //
 // Storage-format conversions and the LinearClamp sampler, written so that every operation is
 // a single IEEE fp32 op in a fixed order (the *_rn intrinsics are never contracted into FMAs,

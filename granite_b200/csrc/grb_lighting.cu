@@ -1,4 +1,4 @@
-// grb_lighting.cu -- clustered deferred lighting as one sm_100a kernel.
+// grb_lighting.cu -- clustered deferred lighting as one sm_90a kernel.
 //
 // Replaces DeferredLightRenderer::render_light (renderer/renderer.cpp:1004-1156), i.e. the two
 // full-screen draws directional.frag and clustering.frag that are additively blended into
@@ -135,18 +135,18 @@ __device__ __forceinline__ int cluster_tile_y(const LightingParams &p, int y)
 {
 	return iclamp(__float2int_rz(fmul(fmul(fadd((float)y, 0.5f), p.inv_res_y), p.xy_scale.y)), 0, p.res_y - 1);
 }
-__device__ __forceinline__ float warp_min_f32(float v)
+// order-preserving float <-> unsigned key (for the integer warp reductions)
+__device__ __forceinline__ unsigned fkey(float f)
 {
-	float r;
-	asm volatile("redux.sync.min.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-	return r;
+	unsigned u = __float_as_uint(f);
+	return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-__device__ __forceinline__ float warp_max_f32(float v)
-{
-	float r;
-	asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-	return r;
-}
+__device__ __forceinline__ float fkey_inv(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k); }
+
+// Float warp min / max of non-NaN values: sm_90 reduces only integers in one instruction
+// (redux.sync.u32), so the floats go through their order-preserving keys.
+__device__ __forceinline__ float warp_min_f32(float v) { return fkey_inv(__reduce_min_sync(0xffffffffu, fkey(v))); }
+__device__ __forceinline__ float warp_max_f32(float v) { return fkey_inv(__reduce_max_sync(0xffffffffu, fkey(v))); }
 
 // World position of a pixel and its cluster coordinates.  The tile index and Z slice are part
 // of the bit-exact contract with the reference (clustering.vert:10-14, clustering.frag:38-39,
@@ -370,21 +370,21 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta) deferred_lighting_kernel(co
 		p.hdr.at(x, y) = __ldg(&p.emissive.at(x, y)); // sky keeps the attachment value
 }
 // ---------------------------------------------------------------------------------------------
-// Two pixels per thread, packed fp32 (FFMA2 / FMUL2 / FADD2 of sm_100).
+// Two pixels per thread in float2 lanes.
 //
-// The pass is bound by instruction issue (ncu: ~80 % issue utilisation, 3 % DRAM), and ~60 % of
-// the issued instructions are fp32 multiply/add.  Blackwell issues TWO fp32 operations per
-// FFMA2-class instruction, so the kernel below carries two horizontally adjacent pixels per
-// thread in float2 lanes: the per-light vector math (light vector, distances, half vector, the
-// three dot products, Fresnel, the GGX terms) is issued once for both, and the per-light
-// control overhead (mask walk, record loads, votes) is amortised over twice the pixels.  A warp
-// covers a 16x4 pixel block, a CTA 64x4.  Results are the same function as the 1-pixel kernel;
-// lanes differ only in fp32 rounding of reassociated terms, far below the B10G11R11 step.
+// The pass is bound by instruction issue, and most of the issued instructions are fp32
+// multiply/add.  The kernel below carries two horizontally adjacent pixels per thread: the
+// per-light control overhead (mask walk, record loads, votes, light-record decoding) is
+// amortised over twice the pixels, and the two pixels' vector math (light vector, distances,
+// half vector, the three dot products, Fresnel, the GGX terms) gives the scheduler two
+// independent dependency chains.  A warp covers a 16x4 pixel block, a CTA 64x4.  Results are
+// the same function as the 1-pixel kernel; lanes differ only in fp32 rounding of reassociated
+// terms, far below the B10G11R11 step.
 using f2 = float2;
 __device__ __forceinline__ f2 mk2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return __ffma2_rn(a, b, c); }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ f2 rsqrt2(f2 a) { return make_float2(rsqrt_fast(a.x), rsqrt_fast(a.y)); }
 __device__ __forceinline__ f2 clamp2(f2 a, float lo, float hi) { return make_float2(fminf(fmaxf(a.x, lo), hi), fminf(fmaxf(a.y, lo), hi)); }
 __device__ __forceinline__ f2 dot3_2(f2 ax, f2 ay, f2 az, f2 bx, f2 by, f2 bz) { return fma2(az, bz, fma2(ay, by, mul2(ax, bx))); }
@@ -782,14 +782,6 @@ __device__ __forceinline__ void light_terms(const SurfaceP &s, const float4 l0, 
 	shade_terms(s, fma2(lx, inv_d, s.Vx), fma2(ly, inv_d, s.Vy), fma2(lz, inv_d, s.Vz), w_pre, a, ga, gb);
 }
 
-// order-preserving float <-> unsigned key (for the integer warp reductions)
-__device__ __forceinline__ unsigned fkey(float f)
-{
-	unsigned u = __float_as_uint(f);
-	return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float fkey_inv(unsigned k) { return __uint_as_float((k & 0x80000000u) ? (k ^ 0x80000000u) : ~k); }
-
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_kernel(const LightingParams p, const PersistentArgs a)
@@ -1078,7 +1070,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 			}
 		}
 
-		// world-space bounding box of the block's lit pixels (float warp reductions: redux.sync.f32, sm_100a)
+		// world-space bounding box of the block's lit pixels (float warp reductions)
 		float bmin_x, bmin_y, bmin_z, bmax_x, bmax_y, bmax_z;
 		{
 			const float kBig = 3.0e38f;

@@ -1,12 +1,12 @@
 // grb_post.cu -- HDR post chain (bloom threshold / pyramid / luminance / tonemap) and post-AA
-// (FXAA, TAA resolve) as sm_100a kernels.  Compiled with -fmad=false: every multiply/add is a
+// (FXAA, TAA resolve) as sm_90a kernels.  Compiled with -fmad=false: every multiply/add is a
 // separate IEEE op in source order, so results are comparable bit-for-bit with the CPU oracle
 // except where a transcendental (log2f, exp2f, powf) is involved.
 //
 // What each kernel replaces in the reference is cited at its entry point.  None of these is a
 // translation of the GLSL: a pass here is one CUDA grid over OUTPUT texels (optionally only the
 // rows of one screen-row shard), reading packed texels straight from HBM/L2 with 4/8-byte
-// coalesced accesses; the small pyramid levels live entirely in the 126 MB L2.
+// coalesced accesses; the small pyramid levels live entirely in the 50 MB L2.
 #include "grb_common.cuh"
 
 #include <cooperative_groups.h>

@@ -1,14 +1,15 @@
 // grb_post_fast.cu -- the full-resolution streaming passes of the post chain (tonemap, FXAA, TAA
-// resolve) arranged for instruction issue, which is what bounds them on B200: at 3840x2160 each
-// of them moves 66 - 265 MB (10 - 40 us at the measured 6.5 TB/s) but the straightforward
-// one-thread-per-pixel forms in grb_post.cu execute 130 - 1750 instructions per pixel.
+// resolve) arranged for instruction issue: at 3840x2160 each of them moves 66 - 265 MB (20 - 80 us
+// at the H100 SXM's 3.35 TB/s data-sheet bandwidth) but the straightforward one-thread-per-pixel
+// forms in grb_post.cu execute 130 - 1750 instructions per pixel.
 //
 // Contract: every output is within 1 unit of its STORED format (8-bit code, B10G11R11 code, fp16
-// ulp) of the reference arithmetic (north_star: "within 1 ULP per channel"), and identical for all
-// but a ~1e-4 fraction of values: the arithmetic is re-associated and uses FMA, the fast
-// reciprocal / log2 / exp2 units and packed FFMA2, none of which moves a result by more than a few
-// fp32 ulps before it is quantised.  (Compiled with FMA contraction on; grb_post.cu keeps the
-// bit-exact forms, selected with GRB_POST_EXACT=1 and used for shapes these kernels do not cover.)
+// ulp) of the reference arithmetic ("within 1 ULP per channel"), and identical for all but a
+// ~1e-4 fraction of values: the arithmetic is re-associated and uses FMA and the fast
+// reciprocal / log2 / exp2 units, none of which moves a result by more than a few fp32 ulps
+// before it is quantised.  Two channels or pixels travel together in float2 lanes (f2 below).
+// (Compiled with FMA contraction on; grb_post.cu keeps the bit-exact forms, selected with
+// GRB_POST_EXACT=1 and used for shapes these kernels do not cover.)
 #include "grb_common.cuh"
 
 #include <cstdlib>
@@ -19,10 +20,11 @@ namespace
 {
 using f2 = float2;
 GRB_DEV f2 mk2(float a) { return make_float2(a, a); }
-GRB_DEV f2 add2(f2 a, f2 b) { return __fadd2_rn(a, b); }
-GRB_DEV f2 sub2(f2 a, f2 b) { return __fadd2_rn(a, make_float2(-b.x, -b.y)); }
-GRB_DEV f2 mul2(f2 a, f2 b) { return __fmul2_rn(a, b); }
-GRB_DEV f2 fma2(f2 a, f2 b, f2 c) { return __ffma2_rn(a, b, c); }
+// plain operators: ptxas may contract a multiply feeding an add into an FFMA, as the contract allows
+GRB_DEV f2 add2(f2 a, f2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+GRB_DEV f2 sub2(f2 a, f2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+GRB_DEV f2 mul2(f2 a, f2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+GRB_DEV f2 fma2(f2 a, f2 b, f2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 // ------------------------------------------------------------------------------- K11 tonemap
 // tonemap.frag:55-66.  One thread = 4 horizontally adjacent pixels of one row.  With the bloom image

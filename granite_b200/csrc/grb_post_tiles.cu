@@ -13,11 +13,9 @@
 //      once instead of once per tap);
 //   3. every output texel then needs 3 column set-ups + 3 row set-ups (the taps' bilinear
 //      footprints are separable) and 36 conflict-free 16-byte shared-memory reads; the arithmetic
-//      is the sampler's fp32 sequence in packed form (two channels per instruction).  ptxas
-//      contracts the packed multiply / add pairs into FFMA2 even when they are written as
-//      mul.rn.f32x2 + add.rn.f32x2 and -fmad=false is given (CUDA 12.9), so a result can differ from
-//      the oracle's unfused sequence in the last fp32 bit: after the fp16 store ~5e-5 of the
-//      texels differ by one fp16 ulp, the rest are identical (north_star's bar: 1 ULP per channel).
+//      is the sampler's fp32 sequence, two channels at a time in float2 lanes.  Each lane is an
+//      explicitly rounded multiply or add (__fmul_rn / __fadd_rn), which ptxas never contracts, so
+//      the sequence is the oracle's unfused one (the tests allow 1 fp16 ULP per channel).
 //
 // The first two passes of the chain are FUSED (grb_bloom_threshold_downsample): the 1/2-resolution
 // threshold image "t" is produced tile by tile in shared memory from a TMA-loaded tile of HDR-main,
@@ -44,8 +42,8 @@ namespace
 {
 using f2 = float2;
 GRB_DEV f2 mk2(float a) { return make_float2(a, a); }
-GRB_DEV f2 add2(f2 a, f2 b) { return __fadd2_rn(a, b); }
-GRB_DEV f2 mul2(f2 a, f2 b) { return __fmul2_rn(a, b); }
+GRB_DEV f2 add2(f2 a, f2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+GRB_DEV f2 mul2(f2 a, f2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // ---------------------------------------------------------------------------------- TMA plumbing
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,

@@ -1,4 +1,4 @@
-// nccl_collectives.hpp -- RenderGraphCollectives over NCCL (NVLink 5 / NVSwitch), one rank per
+// nccl_collectives.hpp -- RenderGraphCollectives over NCCL (NVLink 4 / NVSwitch), one rank per
 // process/GPU.  libnccl is resolved at run time (dlopen of libnccl.so.2 -- the copy PyTorch
 // already loaded when the host process is a torchrun rank), so the host library itself has no
 // link-time NCCL dependency.  The unique id is created on rank 0 and distributed by the caller

@@ -11,7 +11,7 @@
 // What is new: everything below that surface.  There are no barriers, layouts, queues or
 // semaphores to plan -- a baked graph is a topologically ordered list of passes recorded on one
 // CUDA stream per device (stream order IS the dependency), physical images are plain device
-// allocations (no aliasing: 180 GB of HBM3e makes the reference's transient aliasing pointless),
+// allocations (no aliasing: 80 GB of HBM3 makes the reference's transient aliasing pointless),
 // and per-pass GPU timestamps are CUDA events.
 #pragma once
 

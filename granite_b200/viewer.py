@@ -170,8 +170,8 @@ def estimate_band_cost(projection, view, light_positions, light_colors, width, h
 def band_partition_measured(height: int, width: int, world: int, cost_per_4_rows, align: int = 8, post_warp_inst_per_pixel: float = 9.4):
     """Row bands of equal estimated GPU work from Viewer.measure_row_cost() (warp instructions of the
     lighting pass per 4-row group).  The band-proportional part of the post chain (threshold,
-    first down/upsample, tonemap: ~300 thread instructions = 9.4 warp instructions per pixel, from
-    profiles/round1c_frame_launches.md) is added per row so that light-free bands are not free."""
+    first down/upsample, tonemap: ~300 thread instructions = 9.4 warp instructions per pixel, counted
+    with Nsight Compute on an earlier GPU generation) is added per row so that light-free bands are not free."""
     assert align % 4 == 0
     c = np.asarray(cost_per_4_rows, np.float64)
     groups = (height + 3) // 4

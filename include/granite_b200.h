@@ -1,5 +1,5 @@
 /*
- * granite_b200.h -- C ABI of the B200-native executor for Granite's clustered deferred
+ * granite_b200.h -- C ABI of the H100-native executor for Granite's clustered deferred
  * lighting + HDR post chain (libgranite_b200.so).
  *
  * This is the drop-in boundary: every entry point replaces one shader dispatch / draw that

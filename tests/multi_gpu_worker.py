@@ -19,6 +19,16 @@ sys.path.insert(0, ROOT)
 def main():
     w, h, n_lights, fxaa = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4])
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
+    gpus = torch.cuda.device_count()
+    if world > gpus:
+        # More ranks than GPUs: ranks share a device.  NCCL refuses two ranks of one host on one device (it compares
+        # host hash and bus id), so each rank names a host of its own and NCCL connects them through its socket
+        # transport on the loopback interface.  The frame's own exchange -- the downsample kernel's stores into the
+        # IPC-mapped images of every rank, the epoch flags the pyramid tail waits on -- runs unchanged.
+        os.environ["NCCL_HOSTID"] = f"granite-test-rank-{rank}"
+        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
+        os.environ.setdefault("NCCL_IB_DISABLE", "1")
+    local = local % gpus
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     from granite_b200 import synth, viewer

@@ -169,19 +169,37 @@ def test_hdr10_output_rejects_fxaa(built):
     v.close()
 
 
-def test_gtx_reader_reads_the_reference_lookup_textures(built, oracle):
-    """The host library's .gtx reader (host/post/smaa.cpp) against the Python reader the oracle tests use."""
+def _write_gtx(path, fmt, texels):
+    """Granite's memory-mapped texture container (vulkan/texture/memory_mapped_texture.cpp:29-46): 16-byte magic,
+    type, VkFormat, width, height, depth, layers, levels, flags (u32 each), payload size (u64), texels at byte 64."""
+    h, w = texels.shape[:2]
+    hdr = b"GRANITE TEXFMT1\0" + np.array([1, fmt, w, h, 1, 1, 1, 0], "<u4").tobytes() + np.array([texels.nbytes], "<u8").tobytes()
+    with open(path, "wb") as f:
+        f.write(hdr + bytes(64 - len(hdr)) + np.ascontiguousarray(texels).tobytes())
+
+
+def test_gtx_reader_reads_the_reference_lookup_textures(built, oracle, tmp_path):
+    """The host library's .gtx reader (host/post/smaa.cpp) against the Python reader the oracle tests use, on
+    containers holding the payloads of the reference's area.gtx / search.gtx (stored with the SMAA fixture), and
+    on the reference's own files where its assets are present."""
     from granite_b200 import capi, viewer
 
-    if not os.path.isdir(oracle.SMAA_LUT_DIR):
-        pytest.skip("the reference's assets are not on this machine")
-    area, search = oracle.smaa_luts()
-    fmt, a = viewer.load_gtx(os.path.join(oracle.SMAA_LUT_DIR, "area.gtx"))
-    assert fmt == capi.FORMAT_R8G8_UNORM and np.array_equal(a, area)
-    fmt, s = viewer.load_gtx(os.path.join(oracle.SMAA_LUT_DIR, "search.gtx"))
-    assert fmt == capi.FORMAT_R8_UNORM and np.array_equal(s, search)
-    with pytest.raises(RuntimeError):
-        viewer.load_gtx("/nonexistent.gtx")
+    fix = np.load(os.path.join(ROOT, "tests", "golden", "refsmaa_160x96.npz"))
+    cases = [(str(tmp_path / "area.gtx"), capi.FORMAT_R8G8_UNORM, fix["area"]), (str(tmp_path / "search.gtx"), capi.FORMAT_R8_UNORM, fix["search"])]
+    for path, fmt, texels in cases:
+        _write_gtx(path, fmt, texels)
+    if os.path.isdir(oracle.SMAA_LUT_DIR):
+        cases += [(os.path.join(oracle.SMAA_LUT_DIR, "area.gtx"), capi.FORMAT_R8G8_UNORM, fix["area"]),
+                  (os.path.join(oracle.SMAA_LUT_DIR, "search.gtx"), capi.FORMAT_R8_UNORM, fix["search"])]
+    for path, fmt, texels in cases:
+        got_fmt, got = viewer.load_gtx(path)
+        assert got_fmt == fmt and np.array_equal(got, texels), path
+        assert np.array_equal(oracle.load_gtx(path), texels), path
+    short = tmp_path / "short.gtx"
+    short.write_bytes((tmp_path / "search.gtx").read_bytes()[:100])
+    for bad in ("/nonexistent.gtx", str(short)):
+        with pytest.raises(RuntimeError):
+            viewer.load_gtx(bad)
 
 
 def test_band_partition():

@@ -1,8 +1,7 @@
 """Volumetric fog accumulation on the GPU (granite_b200/csrc/grb_fog.cu through the C ABI) against the oracle.  Sorted after the
-validated tests and expected-to-fail-tolerant: written after the round's GPU time had run out.  Verified without a GPU: the
+other GPU tests.  Also verified without a GPU: the
 kernel's source compiled for the CPU, bit for bit with the oracle, and the oracle against the reference's shader
-(tests/test_fog_cpu.py).  On hardware exp2f is CUDA's: the stored fp16 values may differ by one ulp.  An XPASS means the first
-hardware run agreed."""
+(tests/test_fog_cpu.py).  On hardware exp2f is CUDA's: the stored fp16 values may differ by one ulp."""
 import ctypes as C
 
 import numpy as np
@@ -10,7 +9,7 @@ import pytest
 
 from tests.test_fog_cpu import make_density
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: the kernel is verified through CPU emulation of its source only")]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("w,h,d", [(33, 17, 7), (160, 92, 64), (320, 180, 128)])

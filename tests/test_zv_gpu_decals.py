@@ -1,7 +1,7 @@
 """Volumetric-decal binning on the GPU (granite_b200/csrc/grb_decal.cu through the C ABI, and a viewer frame with
-volumetric_decals) against the oracle.  Sorted after the validated tests and expected-to-fail-tolerant: written after the
-round's GPU time had run out.  Verified without a GPU: the kernels' source compiled for the CPU, bit for bit with the oracle,
-and the oracle bit for bit with the reference's shader (tests/test_decal_cpu.py).  An XPASS means the first hardware run agreed."""
+volumetric_decals) against the oracle.  Sorted after the other GPU tests.  Also verified without
+a GPU: the kernels' source compiled for the CPU, bit for bit with the oracle,
+and the oracle bit for bit with the reference's shader (tests/test_decal_cpu.py)."""
 import ctypes as C
 
 import numpy as np
@@ -10,7 +10,7 @@ import pytest
 from tests import common
 from tests.test_decal_cpu import _camera, make_decals
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: the kernels are verified through CPU emulation of their source only")]
+pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("n,res", [(1, (16, 8)), (33, (128, 64)), (300, (128, 64)), (4096, (128, 64))])

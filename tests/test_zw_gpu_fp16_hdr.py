@@ -1,15 +1,15 @@
 """"renderTargetFp16" on the GPU: lighting into, and bloom threshold / tonemap / TAA out of, an R16G16B16A16_SFLOAT HDR-main
 (the fp16 instantiations of the generic kernels, through the C ABI) against the oracle, and a viewer frame with
-render_target_fp16.  Sorted after the validated tests and expected-to-fail-tolerant: written after the round's GPU time had run
-out.  What IS verified without a GPU: the oracle's fp16 paths against the reference's own shaders with the shims' HDR
+render_target_fp16.  Sorted after the other GPU tests.  Also verified without
+a GPU: the oracle's fp16 paths against the reference's own shaders with the shims' HDR
 sampler / blend in that format (tests/test_oracle_ref_fp16_hdr.py); the kernels' B10G11R11 instantiations (same source, the
-texel decode apart) are the ones the validated tests run.  An XPASS means the first hardware run agreed."""
+texel decode apart) are the ones the other GPU tests run."""
 import numpy as np
 import pytest
 
 from tests import common
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: fp16 instantiations of hardware-validated kernels")]
+pytestmark = pytest.mark.gpu
 
 
 def _f16_code_diff(a, b):

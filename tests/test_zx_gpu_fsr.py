@@ -1,9 +1,9 @@
 """FSR 1 on the GPU (granite_b200/csrc/grb_fsr.cu through the C ABI, and a viewer frame with resolution_scale < 1) against the
-oracle and the reference-shader fixture.  Sorted after the validated tests and expected-to-fail-tolerant: these kernels were
-written after the round's GPU time had run out.  What IS verified without a GPU: their source, compiled for the CPU, bit for
+oracle and the reference-shader fixture.  Sorted after the other GPU tests.  Also verified
+without a GPU: their source, compiled for the CPU, bit for
 bit against the oracle (tests/test_fsr_kernel_source_cpu.py), and the oracle bit for bit against the reference's two shaders
 (tests/test_oracle_ref_fsr.py).  What this file adds on hardware: the launch configuration and CUDA's powf in the sRGB
-stores (<= 1 code where a target is sRGB; UNORM targets must be exact).  An XPASS means the first hardware run agreed."""
+stores (<= 1 code where a target is sRGB; UNORM targets must be exact)."""
 import os
 
 import numpy as np
@@ -12,7 +12,7 @@ import pytest
 from tests import common
 from tests.test_oracle_ref_smaa import smaa_test_image
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: the kernels are verified through CPU emulation of their source only")]
+pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 

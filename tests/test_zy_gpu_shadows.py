@@ -1,11 +1,10 @@
 """Shadowed positional lights on the GPU (grb_deferred_lighting_shadowed through the C ABI, and a viewer frame with
-clustered_lights_shadows) against the oracle and the reference-shader fixture.  Sorted after the validated tests and
-expected-to-fail-tolerant: this path was written after the round's GPU time had run out.  What IS verified without a GPU:
+clustered_lights_shadows) against the oracle and the reference-shader fixture.  Sorted after the other GPU tests.
+Also verified without a GPU:
 the comparison samplers' source, compiled for the CPU, bit for bit against the oracle (tests/test_shadow_source_cpu.py);
 the oracle against the reference's own shadowed clustering.frag (tests/test_oracle_ref_light_shadows.py); the host
 clusterer's shadow transforms against the reference's math.  What this file adds on hardware: the shadow branch inside
-the warp-uniform light walk of the generic lighting kernel, the pointer table, the upload.  An XPASS means the first
-hardware run agreed."""
+the warp-uniform light walk of the generic lighting kernel, the pointer table, the upload."""
 import os
 
 import numpy as np
@@ -14,7 +13,7 @@ import pytest
 from tests import common
 from tests.test_oracle_ref_light_shadows import shadow_case
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: verified through CPU emulation of the sampler source and the reference-shader pin of the oracle only")]
+pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 

@@ -1,9 +1,7 @@
 """SMAA on the GPU (granite_b200/csrc/grb_smaa.cu through the C ABI) against the oracle and against the
-reference-shader fixture.  Sorted last on purpose, and expected-to-fail-tolerant: these kernels were written after the
-round's GPU time had run out.  What IS verified is their source, compiled for the CPU and compared bit for bit with
+reference-shader fixture.  Sorted last.  Also verified without a GPU: their source, compiled for the CPU and compared bit for bit with
 the oracle and the reference shaders (tests/test_smaa_kernel_source_cpu.py); what this file adds on hardware is the
-launch configuration, the vector loads and CUDA's powf in the sRGB round trip of the blend pass.  An XPASS here means
-the first hardware run agreed."""
+launch configuration, the vector loads and CUDA's powf in the sRGB round trip of the blend pass."""
 import os
 
 import numpy as np
@@ -12,7 +10,7 @@ import pytest
 from tests import common
 from tests.test_oracle_ref_smaa import smaa_test_image
 
-pytestmark = [pytest.mark.gpu, pytest.mark.xfail(strict=False, reason="first run on hardware: the kernels are verified through CPU emulation of their source only")]
+pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 

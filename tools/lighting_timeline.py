@@ -21,6 +21,7 @@ gcam = harness.camera_struct(cam)
 dev.build(gcam)
 gb = harness.GBufferDevice(scene)
 sched = harness.lighting_schedule(h)
+sms = torch.cuda.get_device_properties(0).multi_processor_count  # one persistent CTA per SM
 for it in range(4):
     hdr = gb.emissive.clone()
     torch.cuda.synchronize()
@@ -32,13 +33,13 @@ for it in range(4):
     capi.lib().grb_debug_lighting_dump(C.c_void_p(blocks.ctypes.data), C.c_void_p(warps.ctypes.data))
     items = np.zeros(256 * 16, np.uint32); last = np.zeros((256 * 16, 8, 2), np.uint32)
     capi.lib().grb_debug_lighting_dump2(C.c_void_p(items.ctypes.data), C.c_void_p(last.ctypes.data))
-    wv = warps[: 148 * 16]
+    wv = warps[: sms * 16]
     start = wv[:, 0].astype(np.int64); start -= start.min()
     end = start + wv[:, 1]
     cyc = blocks[:, 0].astype(np.float64).reshape(540, 240)
     print(f"iter {it} ({'scheduled' if it >= 2 else 'raster' if it == 0 else 'first scheduled (raster order)'}): kernel {e0.elapsed_time(e1) * 1e3:.0f} us; "
           f"warp start spread {start.max() / 1e3:.1f} us; warp end min/median/p90/max = {end.min() / 1e3:.0f}/{np.median(end) / 1e3:.0f}/{np.percentile(end, 90) / 1e3:.0f}/{end.max() / 1e3:.0f} us")
-    per_sm = end.reshape(148, 16).max(1)
+    per_sm = end.reshape(sms, 16).max(1)
     print("   per-SM finish min/median/max us:", per_sm.min() / 1e3, np.median(per_sm) / 1e3, per_sm.max() / 1e3)
     print(f"   block cycles: mean {cyc.mean():.0f} median {np.median(cyc):.0f} p99 {np.percentile(cyc, 99):.0f} max {cyc.max():.0f}; rows with mean > 30000: {(cyc.mean(1) > 30000).sum()}")
     top = np.argsort(-cyc.reshape(-1))[:5]
@@ -47,6 +48,6 @@ for it in range(4):
     for wq in slow:
         k = int(items[wq]); ring = [tuple(int(v) for v in last[wq, (k - j) & 7]) for j in range(min(k, 8))]
         print(f"   straggler warp {wq} (sm {wq // 16}): end {end[wq] / 1e3:.1f} us, {k} items; last fetches (item, us): {[(a, round(b / 1e3, 1)) for a, b in ring]}")
-    print("   items per warp min/median/max:", items[:148 * 16].min(), np.median(items[:148 * 16]), items[:148 * 16].max())
+    print("   items per warp min/median/max:", items[:sms * 16].min(), np.median(items[:sms * 16]), items[:sms * 16].max())
     late = np.argsort(-(blocks[:, 1].astype(np.int64)))[:5]
     print("   latest-started blocks (by, bx, cycles, start us):", [(int(t // 240), int(t % 240), int(blocks[t, 0]), round(blocks[t, 1] / 1e3, 1)) for t in late])
