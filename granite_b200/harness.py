@@ -243,6 +243,18 @@ def smaa_edge_detection(color_t, quality, edges_t, rows=None):
     capi.check(capi.lib().grb_smaa_edge_detection(C.byref(ci), int(quality), C.byref(ei), capi.rows(rows), capi.stream_ptr()), "grb_smaa_edge_detection")
 
 
+def smaa_edge_detection_to_peers(color_t, quality, edge_images, flag_arrays, windows, flag_index, epoch, counter_t, rows=None):
+    """grb_smaa_edge_detection_to_peers with every rank's edge image and flag array as a tensor on this device:
+    edge_images[q]: (H, W, 2) uint8, flag_arrays[q]: int32 tensor, windows[q]: (y0, y1); counter_t: one zeroed int32."""
+    n = len(edge_images)
+    ci, li = capi.image(color_t, capi.FORMAT_R8G8B8A8_UNORM), capi.image(edge_images[0], capi.FORMAT_R8G8_UNORM)
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in edge_images])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    wins = (capi.GrbRows * n)(*[capi.GrbRows(int(a), int(b)) for a, b in windows])
+    capi.check(capi.lib().grb_smaa_edge_detection_to_peers(C.byref(ci), int(quality), C.byref(li), images, flags, wins, n, int(flag_index), int(epoch),
+                                                           _ptr(counter_t), capi.rows(rows), capi.stream_ptr()), "grb_smaa_edge_detection_to_peers")
+
+
 def smaa_blend_weights(edges_t, area_t, search_t, quality, weights_t, rows=None):
     """area_t: (560, 160, 2) uint8, search_t: (16, 64) or (16, 64, 1) uint8, weights_t: (H, W) int32."""
     ei, ai = capi.image(edges_t, capi.FORMAT_R8G8_UNORM), capi.image(area_t, capi.FORMAT_R8G8_UNORM)

@@ -28,6 +28,8 @@ public:
 	// Peer-memory exchange: two image slots + a flag array per rank, cudaIpc-mapped into every
 	// other rank (handles are exchanged with one ncclAllGather).  GRB_SHARD_EXCHANGE=nccl disables it.
 	bool peer_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
+	// Second channel, same set-up and teardown: the SMAA edge rows (host/post/smaa.cpp).
+	bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
 
 private:
 	bool collective_failed(const char *what);
@@ -44,8 +46,11 @@ private:
 		uint32_t *flags[8] = {};
 		std::vector<void *> opened;
 		uint32_t epoch = 0;
-	} peer;
-	bool setup_peer_exchange(size_t image_bytes);
-	void release_peer_exchange();
+	};
+	PeerState bloom_d0;  // bloom d0 bands
+	PeerState smaa_edge; // SMAA edge rows
+	bool begin_frame(PeerState &channel, size_t image_bytes, PeerSlot &slot);
+	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
+	void release_peer_exchange(PeerState &channel);
 };
 } // namespace Granite

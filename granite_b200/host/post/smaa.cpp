@@ -1,5 +1,11 @@
 // smaa.cpp -- "smaa-edge" / "smaa-weights" / "smaa-blend" pass builders (renderer/post/smaa.cpp:32-209), the lookup
 // textures they sample and the .gtx reader for them.
+//
+// Row-sharded frames (shard_plan.hpp derives the rows): a rank detects the edges of its own rows, and its weight pass
+// needs a window of up to 2 * max_search_steps + 6 rows around its band, mostly other ranks' rows.  The edge kernel
+// stores each row straight into the edge image of every rank whose window holds it (NVLink peer memory, the SMAA
+// channel of RenderGraphCollectives) and raises a flag; the weight pass waits for every rank's flag and reads that
+// copy.  Without peer memory: the plain edge kernel, then the ranks' edge bands are all-gathered with NCCL.
 #include "smaa.hpp"
 
 #include <cuda_runtime.h>
@@ -7,6 +13,7 @@
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <stdexcept>
 
@@ -38,7 +45,10 @@ bool set_smaa_lookup_textures(Vulkan::Device &device, const uint8_t *area_rg8, c
 	info.height = kSearchH;
 	info.format = VK_FORMAT_R8_UNORM;
 	l.search = device.create_image(info);
-	// once per device, before the first frame: plain synchronous copies
+	// once per device, before the first frame: plain synchronous copies.  create_image zero-fills on the device's
+	// stream, which the legacy-stream copies below do not wait for: finish the fill first, or it can land after the
+	// upload and leave zero lookup textures (no SMAA weights at all).
+	device.wait_idle();
 	if (!Vulkan::cuda_ok(cudaMemcpy(l.area->get_device_pointer(), area_rg8, (size_t)kAreaW * kAreaH * 2, cudaMemcpyHostToDevice), "SMAA area texture upload") ||
 	    !Vulkan::cuda_ok(cudaMemcpy(l.search->get_device_pointer(), search_r8, (size_t)kSearchW * kSearchH, cudaMemcpyHostToDevice), "SMAA search texture upload"))
 		return false;
@@ -147,8 +157,6 @@ void setup_smaa_postprocess(RenderGraph &graph, TemporalJitter &jitter, float, c
 {
 	if (preset == SMAAPreset::Ultra_T2X)
 		throw std::logic_error("SMAA T2X (two jittered frames + smaa-t2x-resolve) is not built by this executor.");
-	if (graph.is_sharded() && graph.get_shard_count() > 1)
-		throw std::logic_error("SMAA is not available in row-sharded graphs: its searches cross band borders.");
 	const int quality = preset == SMAAPreset::Low ? 0 : (preset == SMAAPreset::Medium ? 1 : (preset == SMAAPreset::High ? 2 : 3));
 	jitter.init(TemporalJitter::Type::None, vec2(1.0f)); // smaa.cpp:66-67
 
@@ -179,12 +187,47 @@ void setup_smaa_postprocess(RenderGraph &graph, TemporalJitter &jitter, float, c
 	auto &blend_input = smaa_blend.add_texture_input(input);
 	auto &blend_weights = smaa_blend.add_texture_input("smaa-weights");
 
-	smaa_edge.set_build_render_pass([&graph, &edge_out, &edge_input, quality](Vulkan::CommandBuffer &cmd) {
+	// this frame's slot of the edge exchange, from the edge pass to the weight pass (both on the post-graphics stream)
+	struct EdgeExchange
+	{
+		bool peer_stores = false;
+		RenderGraphCollectives::PeerSlot slot;
+	};
+	auto exchange = std::make_shared<EdgeExchange>();
+	smaa_edge.set_build_render_pass([&graph, &edge_out, &edge_input, quality, exchange](Vulkan::CommandBuffer &cmd) {
 		GrbImage color = graph.get_physical_texture_resource(edge_input).as_grb_unorm();
-		GrbImage edges = graph.get_physical_texture_resource(edge_out).as_grb();
-		cmd.check(grb_smaa_edge_detection(&color, quality, &edges, GrbRows{ 0, 0 }, cmd.get_stream_handle()), "grb_smaa_edge_detection");
+		auto &edge_view = graph.get_physical_texture_resource(edge_out);
+		GrbImage edges = edge_view.as_grb();
+		void *stream = cmd.get_stream_handle();
+		const bool sharded = graph.is_sharded() && graph.get_shard_count() > 1;
+		exchange->peer_stores = sharded &&
+		                        graph.get_collectives()->smaa_edge_exchange_begin_frame((size_t)edges.row_pitch * (size_t)edges.height, exchange->slot);
+		if (!sharded)
+		{
+			cmd.check(grb_smaa_edge_detection(&color, quality, &edges, GrbRows{ 0, 0 }, stream), "grb_smaa_edge_detection");
+			return;
+		}
+		const unsigned ranks = graph.get_shard_count();
+		std::vector<GrbRows> windows, bands;
+		for (unsigned r = 0; r < ranks; r++)
+		{
+			const ShardPlan p = graph.get_shard_plan(r);
+			windows.push_back(p.smaa_edge_window);
+			bands.push_back(p.smaa_edges);
+		}
+		const unsigned self = graph.get_shard_rank();
+		if (exchange->peer_stores)
+		{
+			const auto &slot = exchange->slot;
+			cmd.check(grb_smaa_edge_detection_to_peers(&color, quality, &edges, slot.images, slot.flags, windows.data(), (int32_t)slot.count, (int32_t)self,
+			                                           slot.epoch, slot.counter, bands[self], stream),
+			          "grb_smaa_edge_detection_to_peers");
+			return;
+		}
+		cmd.check(grb_smaa_edge_detection(&color, quality, &edges, bands[self], stream), "grb_smaa_edge_detection");
+		graph.get_collectives()->all_gather_rows(cmd, edge_view, bands);
 	});
-	smaa_weight.set_build_render_pass([&graph, &weight_out, &weight_input, quality](Vulkan::CommandBuffer &cmd) {
+	smaa_weight.set_build_render_pass([&graph, &weight_out, &weight_input, quality, exchange](Vulkan::CommandBuffer &cmd) {
 		GrbImage edges = graph.get_physical_texture_resource(weight_input).as_grb();
 		GrbImage weights = graph.get_physical_texture_resource(weight_out).as_grb();
 		GrbImage area, search;
@@ -193,13 +236,24 @@ void setup_smaa_postprocess(RenderGraph &graph, TemporalJitter &jitter, float, c
 			Vulkan::log_error("smaa-weights: no lookup textures on this device (set_smaa_lookup_textures / load_smaa_lookup_textures).\n");
 			return;
 		}
-		cmd.check(grb_smaa_blend_weights(&edges, &area, &search, quality, &weights, GrbRows{ 0, 0 }, cmd.get_stream_handle()), "grb_smaa_blend_weights");
+		void *stream = cmd.get_stream_handle();
+		const bool sharded = graph.is_sharded() && graph.get_shard_count() > 1;
+		if (sharded && exchange->peer_stores)
+		{
+			const auto &slot = exchange->slot;
+			const unsigned self = graph.get_shard_rank();
+			cmd.check(grb_peer_wait(slot.flags[self], (int32_t)slot.count, slot.epoch, stream), "grb_peer_wait");
+			edges.data = slot.images[self]; // the exchanged copy
+		}
+		const GrbRows rows = sharded ? graph.get_shard_plan().smaa_weights : GrbRows{ 0, 0 };
+		cmd.check(grb_smaa_blend_weights(&edges, &area, &search, quality, &weights, rows, stream), "grb_smaa_blend_weights");
 	});
 	smaa_blend.set_build_render_pass([&graph, &blend_out, &blend_input, &blend_weights](Vulkan::CommandBuffer &cmd) {
 		GrbImage color = graph.get_physical_texture_resource(blend_input).as_grb_unorm();
 		GrbImage weights = graph.get_physical_texture_resource(blend_weights).as_grb();
 		GrbImage out = graph.get_physical_texture_resource(blend_out).as_grb(); // SMAA_TARGET_SRGB follows the output format (smaa.cpp:193-194)
-		cmd.check(grb_smaa_neighborhood_blend(&color, &weights, &out, GrbRows{ 0, 0 }, cmd.get_stream_handle()), "grb_smaa_neighborhood_blend");
+		const GrbRows rows = graph.is_sharded() && graph.get_shard_count() > 1 ? graph.get_shard_plan().smaa_blend : GrbRows{ 0, 0 };
+		cmd.check(grb_smaa_neighborhood_blend(&color, &weights, &out, rows, cmd.get_stream_handle()), "grb_smaa_neighborhood_blend");
 	});
 }
 } // namespace Granite

@@ -70,6 +70,14 @@ public:
 		(void)slot;
 		return false;
 	}
+	// The same exchange on a second, independent channel (its own two slots, flag arrays, counter and epoch) for the
+	// SMAA edge rows, which a frame exchanges besides the bloom d0 bands (host/post/smaa.cpp).
+	virtual bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+	{
+		(void)image_bytes;
+		(void)slot;
+		return false;
+	}
 };
 
 class RenderPassInterface
@@ -461,12 +469,14 @@ public:
 	// Row-sharded frames (multi-GPU, one graph per device/process): `bands[r]` = backbuffer rows
 	// [y0, y1) owned by rank r; they must tile the frame.  Builders scale the local band per
 	// resource with shard_rows_for(); an unsharded graph returns {0,0} (= all rows).
-	void set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives, bool fxaa_downstream = false);
+	// smaa_quality_downstream: the SMAA preset (0..3) after the tonemap, -1 for none (it widens the tonemap rows).
+	void set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives, bool fxaa_downstream = false,
+	                    int smaa_quality_downstream = -1);
 	// Rows of every stage for `rank` (this rank by default); whole images when unsharded.
 	ShardPlan get_shard_plan() const { return get_shard_plan(shard_rank); }
 	ShardPlan get_shard_plan(unsigned rank) const
 	{
-		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa);
+		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality);
 	}
 	GrbRows shard_rows_for(unsigned resource_height, unsigned halo_rows = 0) const;
 	GrbRows shard_rows_for_rank(unsigned rank, unsigned resource_height, unsigned halo_rows = 0) const;
@@ -527,6 +537,7 @@ private:
 	std::vector<GrbRows> shard_bands;
 	unsigned shard_rank = 0;
 	bool shard_fxaa = false;
+	int shard_smaa_quality = -1;
 	RenderGraphCollectives *collectives = nullptr;
 
 	RenderTextureResource &get_or_create_texture(const std::string &name);

@@ -88,12 +88,13 @@ struct GrbhViewer
 	int render_height() const { return upscales() ? std::max(int(std::ceil(config.resolution_scale * float(config.height))), 1) : config.height; }
 	bool uses_fxaa() const { return config.post_aa == GRBH_AA_FXAA || config.post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA; }
 	bool uses_smaa() const { return config.post_aa >= GRBH_AA_SMAA_LOW && config.post_aa <= GRBH_AA_SMAA_ULTRA; }
+	int smaa_quality() const { return uses_smaa() ? config.post_aa - GRBH_AA_SMAA_LOW : -1; }
 
 	// rows of the full-resolution inputs this rank must hold: its band + the halo the bloom
 	// threshold (and FXAA through the tonemap) reaches into
 	GrbRows input_rows() const
 	{
-		return compute_shard_plan((unsigned)render_width(), (unsigned)render_height(), bands, rank, uses_fxaa()).lighting;
+		return compute_shard_plan((unsigned)render_width(), (unsigned)render_height(), bands, rank, uses_fxaa(), smaa_quality()).lighting;
 	}
 
 	void upload_rows(Vulkan::CommandBuffer &cmd, RenderTextureResource *res, const void *host, unsigned texel)
@@ -126,7 +127,7 @@ void GrbhViewer::bake_render_graph()
 	dim.format = VK_FORMAT_R8G8B8A8_SRGB; // headless swapchain format (application_headless.cpp:207)
 	graph.set_backbuffer_dimensions(dim);
 	if (!bands.empty())
-		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa());
+		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa(), smaa_quality());
 
 	// scene.add_render_passes(graph) -> LightClusterer::add_render_passes
 	cluster.set_resolution((unsigned)config.cluster_res[0], (unsigned)config.cluster_res[1], (unsigned)config.cluster_res[2]);
@@ -663,6 +664,20 @@ extern "C" int32_t grbh_shard_plan(int32_t width, int32_t height, const GrbRows 
 	const GrbRows all[8] = { p.own, p.fxaa, p.tonemap, p.upsample0, p.downsample0, p.threshold, p.lighting, p.lum_grid };
 	for (int i = 0; i < 8; i++)
 		out9[i] = all[i];
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_shard_plan_smaa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t quality, GrbRows *out6)
+{
+	if (width <= 0 || height <= 0 || count < 0 || (count && !bands) || !out6 || (count && (rank < 0 || rank >= count)) || quality < 0 || quality > 3)
+		return fail("grbh_shard_plan_smaa: bad arguments");
+	GRBH_TRY
+	std::vector<GrbRows> b(bands, bands + count);
+	ShardPlan p = compute_shard_plan((unsigned)width, (unsigned)height, b, (unsigned)rank, false, quality);
+	const GrbRows all[6] = { p.smaa_blend, p.smaa_weights, p.smaa_edges, p.smaa_edge_window, p.tonemap, p.lighting };
+	for (int i = 0; i < 6; i++)
+		out6[i] = all[i];
 	return 0;
 	GRBH_CATCH
 }

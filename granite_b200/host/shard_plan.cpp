@@ -28,9 +28,11 @@ GrbRows scale_band(GrbRows band, unsigned from_h, unsigned to_h)
 }
 } // namespace
 
-ShardPlan compute_shard_plan(unsigned, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa)
+ShardPlan compute_shard_plan(unsigned, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality)
 {
 	ShardPlan p = {};
+	const GrbRows whole = { 0, (int)height };
+	p.smaa_blend = p.smaa_weights = p.smaa_edges = p.smaa_edge_window = whole;
 	const unsigned h_half = ceil_scale(height, 0.5f), h_quarter = ceil_scale(height, 0.25f);
 	const unsigned h_d3 = ceil_scale(height, 0.03125f), h_grid = h_d3 / 2;
 	if (bands.size() <= 1)
@@ -45,6 +47,15 @@ ShardPlan compute_shard_plan(unsigned, unsigned height, const std::vector<GrbRow
 	p.own = bands[rank];
 	p.fxaa = p.own;
 	p.tonemap = fxaa ? clamp_rows(p.own.y0 - 6, p.own.y1 + 6, height) : p.own;
+	if (smaa_quality >= 0)
+	{
+		// derivation in shard_plan.hpp
+		const int steps = 4 << std::min(smaa_quality, 3);
+		p.smaa_blend = p.smaa_edges = p.own;
+		p.smaa_weights = clamp_rows(p.own.y0 - 1, p.own.y1 + 2, height);
+		p.smaa_edge_window = clamp_rows(p.smaa_weights.y0 - (2 * steps + 2), p.smaa_weights.y1 + 2 * steps + 4, height);
+		p.tonemap = clamp_rows(p.own.y0 - 3, p.own.y1 + 2, height);
+	}
 	p.upsample0 = clamp_rows(p.tonemap.y0 / 4 - 1, (p.tonemap.y1 + 3) / 4 + 1, h_quarter);
 	p.downsample0 = scale_band(p.own, height, h_quarter);
 	p.threshold = clamp_rows(2 * p.downsample0.y0 - 2, 2 * p.downsample0.y1 + 2, h_half);

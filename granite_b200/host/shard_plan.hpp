@@ -8,6 +8,27 @@
 //   d0 (1/4)  : 9-tap tent, +-1.75 texels of threshold around 2y+1 + bilinear   -> t rows 2y-2 .. 2y+3
 //   threshold : bilinear of HDR at 2y+1                                         -> HDR rows 2y .. 2y+1 (+-1)
 // Bands are aligned to 64 full-res rows, so the 1/4-res d0 bands tile that level exactly.
+//
+// SMAA 1x (grb_smaa.cu), preset with s = max_search_steps (4 / 8 / 16 / 32 for Low .. Ultra).  Every sample is a
+// bilinear tap of a coordinate computed in fp32.  A tap whose nominal position is a texel centre (an integer row
+// offset) can, after rounding, land a few ulp off it and then takes the neighbouring row with a weight of rounding
+// size; such a row is counted below ("guard row"): in a sharded frame it would otherwise hold another frame's or
+// another rank's bytes, and a weight of 1e-7 can still flip a tie or an 8-bit rounding.  Taps at quarter-row
+// offsets (the searches) read exactly the two rows around them.
+//   blend     : weights at +0 and +1 row (the .w / .y taps of the pixel to the right / below), colour at +-1 row
+//               -> weights rows y-1 .. y+2, colour rows y-2 .. y+2 (guard rows included)
+//   weights   : vertical edge, up search: taps at y - 1/4 - 2k, k = 0 .. s (the end test compares the accumulated
+//               coordinate with one computed in one step, so rounding can allow one step more than s)
+//               -> rows down to y-1-2s; the end tap (1.25 .. 3.25 rows back, integer for the lookup texture's values)
+//               and the corner taps there -> y-2-2s with its guard row.
+//               down search: taps at y + 5/4 + 2k -> rows up to y+2+2s; end tap + 1 row and corner taps
+//               -> y+3+2s, y+4+2s with its guard row.
+//               horizontal edge (+-2 rows with corners) and diagonal searches (<= 16 + 3 rows, High / Ultra only)
+//               reach less.  -> edge rows y - (2s+2) .. y + (2s+4)
+//   edges     : L at -2 .. +1 rows (Ltoptop, Lbottom)           -> colour rows y-3 .. y+2 (guard rows included)
+// So a rank that owns rows [y0, y1) produces the edges of [y0, y1) only; its weight pass runs on [y0-1, y1+2) and
+// reads the edge window [y0-2s-3, y1+2s+6), which the ranks owning those rows deliver (grb_smaa_edge_detection_to_peers);
+// blend writes [y0, y1); the tonemap covers [y0-3, y1+2).  All clamped to the image (taps clamp to the edge rows).
 #pragma once
 
 #include <vector>
@@ -26,7 +47,13 @@ struct ShardPlan
 	GrbRows threshold;  // rows of "threshold" (1/2)
 	GrbRows lighting;   // rows of "HDR-main" (= rows of the G-buffer that must be resident)
 	GrbRows lum_grid;   // rows of the (d3/2) luminance grid this rank samples
+	// SMAA (smaa_quality >= 0); whole images when unsharded or without SMAA
+	GrbRows smaa_blend;       // rows of the SMAA output (= own)
+	GrbRows smaa_weights;     // rows of "smaa-weights" the blend reads
+	GrbRows smaa_edges;       // rows of "smaa-edge" this rank produces (= own)
+	GrbRows smaa_edge_window; // rows of "smaa-edge" the weight pass reads: delivered by the ranks that own them
 };
 
-ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa);
+// smaa_quality: SMAA preset 0..3 (Low .. Ultra) downstream of the tonemap, -1 for none.
+ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1);
 } // namespace Granite

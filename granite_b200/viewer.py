@@ -229,6 +229,18 @@ def shard_plan(width, height, bands, rank, fxaa=False) -> dict:
     return {k: (out[i].y0, out[i].y1) for i, k in enumerate(PLAN_FIELDS)}
 
 
+SMAA_PLAN_FIELDS = ("blend", "weights", "edges", "edge_window", "tonemap", "lighting")
+
+
+def shard_plan_smaa(width, height, bands, rank, quality) -> dict:
+    """SMAA rows one rank computes for preset `quality` 0..3 (host math of granite_b200/host/shard_plan.cpp): the
+    rows it blends, weighs and detects edges on, the edge window its weight pass reads, and its tonemap / lighting rows."""
+    arr = (capi.GrbRows * max(len(bands), 1))(*[capi.GrbRows(a, b) for a, b in bands])
+    out = (capi.GrbRows * 6)()
+    _check(lib().grbh_shard_plan_smaa(width, height, arr, len(bands), rank, int(quality), out), "grbh_shard_plan_smaa")
+    return {k: (out[i].y0, out[i].y1) for i, k in enumerate(SMAA_PLAN_FIELDS)}
+
+
 class Viewer:
     def __init__(self, width, height, post_aa=AA_NONE, hdr_bloom=True, dynamic_exposure=True, cuda_device=0,
                  cluster_res=(128, 64, 4096), timestamps=False, stream=None, pipelined_io=False, hdr10_output=False, hdr10_max_cll=1000.0,

@@ -374,6 +374,19 @@ int32_t grb_smaa_edge_detection(const GrbImage *color, int32_t quality, const Gr
 int32_t grb_smaa_blend_weights(const GrbImage *edges, const GrbImage *area, const GrbImage *search, int32_t quality,
                                const GrbImage *weights, GrbRows rows, void *stream);
 int32_t grb_smaa_neighborhood_blend(const GrbImage *color, const GrbImage *weights, const GrbImage *out, GrbRows rows, void *stream);
+/* grb_smaa_edge_detection of the rows [rows.y0, rows.y1) a rank owns in a row-sharded frame, fused with the exchange
+ * its peers' weight passes need: each texel (the values of grb_smaa_edge_detection) is stored into
+ * peer_images[flag_index] (this rank's own copy) and into peer_images[q] of every rank q whose edge window
+ * peer_windows[q] holds its row.  peer_images[q] is the base address, valid on this device, of rank q's edge image
+ * (cudaIpc-mapped peer memory), all with edges_layout's size and pitch (edges_layout->data is not used).  Then
+ * flags[flag_index] = epoch is release-stored into the flag array of EVERY rank; the consumer is grb_peer_wait on all
+ * peer_count flags before grb_smaa_blend_weights.  scratch_counter: one zero-initialised uint32 in local device memory.
+ * GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1,
+ * a window outside the image; GRB_ERR_UNSUPPORTED_FORMAT: formats, sizes or quality as for grb_smaa_edge_detection.
+ * No reference equivalent (the reference never splits a frame). */
+int32_t grb_smaa_edge_detection_to_peers(const GrbImage *color, int32_t quality, const GrbImage *edges_layout, void *const *peer_images,
+                                         uint32_t *const *peer_flags, const GrbRows *peer_windows, int32_t peer_count, int32_t flag_index,
+                                         uint32_t epoch, uint32_t *scratch_counter, GrbRows rows, void *stream);
 
 /* FidelityFX FSR 1 after the post chain (renderer/post/aa.cpp:75-174 setup_after_post_chain_upscaling;
  * assets/shaders/post/ffx-fsr/{upscale,sharpen}.frag over ffx_fsr1.h, 32-bit paths).

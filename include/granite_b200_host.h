@@ -138,6 +138,10 @@ int32_t grbh_viewer_measure_row_cost(GrbhViewer *viewer, uint32_t *out, int32_t 
 /* The row plan of one rank of a row-sharded frame (granite_b200/host/shard_plan.hpp): out8 =
  * {own, fxaa, tonemap, upsample0, downsample0, threshold, lighting, lum_grid}.  Pure host math. */
 int32_t grbh_shard_plan(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out8);
+/* The SMAA rows of the same plan for preset `quality` 0..3 (Low .. Ultra): out6 = {blend, weights, edges (the rows
+ * this rank produces), edge window (the rows its weight pass reads, delivered by the ranks that own them), tonemap,
+ * lighting}.  Whole images when count <= 1.  Pure host math. */
+int32_t grbh_shard_plan_smaa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t quality, GrbRows *out6);
 
 /* bake_render_graph: declares the passes, bakes, allocates attachments. */
 int32_t grbh_viewer_bake(GrbhViewer *viewer);
