@@ -616,14 +616,17 @@ struct Mat4
 	float m[16];
 };
 
-template <int Quality, bool History, typename HdrTexel = uint32_t>
-__global__ void __launch_bounds__(kBlockX *kBlockY) taa_kernel(TaaInputsT<HdrTexel> in, Mat4 reproj, View<uint32_t> out_color, View<uint2> out_history, int y0,
-                                                              int y1, float4 rt)
+// The two outputs of one TAA texel: colour (B10G11R11) and history (RGBA16F).
+struct TaaTexel
 {
-	int x = blockIdx.x * kBlockX + threadIdx.x;
-	int y = y0 + blockIdx.y * kBlockY + threadIdx.y;
-	if (x >= out_color.w || y >= y1)
-		return;
+	uint32_t color;
+	uint2 history;
+};
+
+// taa_resolve.frag for pixel (x, y).  Shared by taa_kernel and taa_peers_kernel, so both store the same values.
+template <int Quality, bool History, typename HdrTexel>
+__device__ __forceinline__ TaaTexel taa_texel(const TaaInputsT<HdrTexel> &in, const Mat4 &reproj, float4 rt, int x, int y)
+{
 	const int w = in.hdr.w, h = in.hdr.h;
 #define GRB_CUR(DX, DY) hdr_to_taa(fetch_hdr_clamped(in.hdr, x + (DX), y + (DY)))
 	float3 current = GRB_CUR(0, 0);
@@ -727,8 +730,60 @@ __global__ void __launch_bounds__(kBlockX *kBlockY) taa_kernel(TaaInputsT<HdrTex
 	}
 #undef GRB_CUR
 	float3 color = taa_to_hdr(out_c);
-	out_color.at(x, y) = pack_r11g11b10(color.x, color.y, color.z);
-	out_history.at(x, y) = pack_rgba16f(make_float4(out_c.x, out_c.y, out_c.z, 1.0f));
+	return TaaTexel{ pack_r11g11b10(color.x, color.y, color.z), pack_rgba16f(make_float4(out_c.x, out_c.y, out_c.z, 1.0f)) };
+}
+
+template <int Quality, bool History, typename HdrTexel = uint32_t>
+__global__ void __launch_bounds__(kBlockX *kBlockY) taa_kernel(TaaInputsT<HdrTexel> in, Mat4 reproj, View<uint32_t> out_color, View<uint2> out_history, int y0,
+                                                              int y1, float4 rt)
+{
+	int x = blockIdx.x * kBlockX + threadIdx.x;
+	int y = y0 + blockIdx.y * kBlockY + threadIdx.y;
+	if (x >= out_color.w || y >= y1)
+		return;
+	const TaaTexel t = taa_texel<Quality, History>(in, reproj, rt, x, y);
+	out_color.at(x, y) = t.color;
+	out_history.at(x, y) = t.history;
+}
+
+// Row-sharded frames: a texel's history read (at uv - mv) can land on any row, so every rank needs the whole history
+// of the last frame.  Each rank resolves its TAA rows [y0, y1) (colour into its own image) and stores the history of
+// its own rows [own0, own1) into the history slot of every rank, its own included (plain 8-byte stores to IPC-mapped
+// peer memory over NVLink), then publishes "history rows of frame <epoch> landed" in every rank's flag array -- the
+// protocol of bloom_downsample_peers_kernel.  The consumer side is grb_peer_wait before the next frame's resolve.
+template <int Quality, bool History, typename HdrTexel = uint32_t>
+__global__ void __launch_bounds__(kBlockX *kBlockY) taa_peers_kernel(TaaInputsT<HdrTexel> in, Mat4 reproj, View<uint32_t> out_color, PeerTargets targets,
+                                                                    int pitch_texels, int y0, int y1, int own0, int own1, float4 rt, int flag_index,
+                                                                    uint32_t epoch, unsigned *ctas_done)
+{
+	const int x = blockIdx.x * kBlockX + threadIdx.x;
+	const int y = y0 + blockIdx.y * kBlockY + threadIdx.y;
+	if (x < out_color.w && y < y1)
+	{
+		const TaaTexel t = taa_texel<Quality, History>(in, reproj, rt, x, y);
+		out_color.at(x, y) = t.color;
+		if (y >= own0 && y < own1)
+		{
+			const size_t at = (size_t)y * pitch_texels + x;
+			for (int r = 0; r < targets.count; r++)
+				targets.data[r][at] = t.history;
+		}
+	}
+	// as bloom_downsample_peers_kernel: the last CTA to arrive raises this rank's flag on every rank.  Each CTA's history
+	// reads are done before it arrives, so the flag also says "this rank has finished reading last frame's slot".
+	__threadfence_system();
+	__syncthreads();
+	if (threadIdx.x == 0 && threadIdx.y == 0)
+	{
+		const unsigned total = gridDim.x * gridDim.y;
+		if (atomicAdd(ctas_done, 1u) == total - 1u)
+		{
+			*ctas_done = 0u;
+			__threadfence_system();
+			for (int r = 0; r < targets.count; r++)
+				store_release_system(targets.flags[r] + flag_index, epoch);
+		}
+	}
 }
 
 // ------------------------------------------------------------------------------- pyramid tail
@@ -1213,10 +1268,13 @@ extern "C" int32_t grb_taa_resolve(const GrbImage *hdr, const GrbImage *depth, c
 		set_last_error("grb_taa_resolve: quality must be 0..2");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	// GRB_TAA_TILES=1 applies to whole-frame calls (rows {0, 0}) only: a row-sharded frame passes its rows and must
+	// compute the exact kernel's values, which grb_taa_resolve_to_peers computes on the other ranks
+	const bool whole_frame = rows.y0 == 0 && rows.y1 == 0;
 	rows = full_rows(rows, hdr->height);
 	if (rows.y1 <= rows.y0)
 		return GRB_OK;
-	if (history && quality == 2 && !hdr16)
+	if (history && quality == 2 && !hdr16 && whole_frame)
 	{
 		int32_t rc = GRB_OK;
 		if (launch_taa_fast(hdr, depth, mv, history, reproj16, out_color, out_history, rows, as_stream(stream), &rc))
@@ -1268,6 +1326,113 @@ extern "C" int32_t grb_taa_resolve(const GrbImage *hdr, const GrbImage *depth, c
 		GRB_LAUNCH(2, true);
 #undef GRB_LAUNCH
 	return check_launch("grb_taa_resolve");
+}
+
+extern "C" int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage *depth, const GrbImage *mv, const GrbImage *history, const float *reproj16,
+                                            int32_t quality, const GrbImage *out_color, const GrbImage *history_layout, void *const *peer_images,
+                                            uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter,
+                                            GrbRows rows, GrbRows own, void *stream)
+{
+	const bool hdr16 = image_ok(hdr, GRB_FORMAT_R16G16B16A16_SFLOAT, 8);
+	if ((!hdr16 && !image_ok(hdr, GRB_FORMAT_B10G11R11_UFLOAT_PACK32, 4)) || !image_ok(out_color, GRB_FORMAT_B10G11R11_UFLOAT_PACK32, 4) || !history_layout ||
+	    history_layout->format != GRB_FORMAT_R16G16B16A16_SFLOAT || history_layout->row_pitch < history_layout->width * 8 || (history_layout->row_pitch % 8) != 0 ||
+	    out_color->width != hdr->width || out_color->height != hdr->height || history_layout->width != hdr->width || history_layout->height != hdr->height)
+	{
+		set_last_error("grb_taa_resolve_to_peers: hdr B10G11R11_UFLOAT or R16G16B16A16_SFLOAT, out_color B10G11R11_UFLOAT, history layout R16G16B16A16_SFLOAT, equal sizes");
+		return GRB_ERR_UNSUPPORTED_FORMAT;
+	}
+	if (history && (!image_ok(history, GRB_FORMAT_R16G16B16A16_SFLOAT, 8) || !image_ok(depth, GRB_FORMAT_D32_SFLOAT, 4) ||
+	                !image_ok(mv, GRB_FORMAT_R16G16_SFLOAT, 4) || !reproj16 || history->width != hdr->width || history->height != hdr->height ||
+	                depth->width != hdr->width || depth->height != hdr->height || mv->width != hdr->width || mv->height != hdr->height))
+	{
+		set_last_error("grb_taa_resolve_to_peers: with history, depth (D32_SFLOAT), mv (R16G16_SFLOAT) and reproj are required");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (quality < 0 || quality > 2)
+	{
+		set_last_error("grb_taa_resolve_to_peers: quality must be 0..2");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (!peer_images || !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0 || flag_index >= peer_count)
+	{
+		set_last_error("grb_taa_resolve_to_peers: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	PeerTargets targets{};
+	targets.count = peer_count;
+	for (int r = 0; r < peer_count; r++)
+	{
+		if (!peer_images[r] || !peer_flags[r])
+		{
+			set_last_error("grb_taa_resolve_to_peers: null peer pointer");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+		if (history && history->data == peer_images[r])
+		{
+			set_last_error("grb_taa_resolve_to_peers: the history input must be distinct from every peer image");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+		targets.data[r] = static_cast<uint2 *>(peer_images[r]);
+		targets.flags[r] = peer_flags[r];
+	}
+	rows = full_rows(rows, hdr->height);
+	if (own.y0 == 0 && own.y1 == 0)
+		own.y1 = hdr->height;
+	if (own.y0 < 0 || own.y1 < own.y0 || own.y1 > hdr->height || own.y0 < rows.y0 || own.y1 > rows.y1)
+	{
+		set_last_error("grb_taa_resolve_to_peers: own rows must lie inside rows and the image");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	TaaInputs in{};
+	in.hdr = view_of<const uint32_t>(hdr);
+	Mat4 m{};
+	if (history)
+	{
+		in.depth = view_of<const float>(depth);
+		in.mv = view_of<const uint32_t>(mv);
+		in.history = view_of<const uint2>(history);
+		for (int i = 0; i < 16; i++)
+			m.m[i] = reproj16[i];
+	}
+	auto oc = view_of<uint32_t>(out_color);
+	float4 rt = make_float4(1.0f / (float)hdr->width, 1.0f / (float)hdr->height, (float)hdr->width, (float)hdr->height);
+	// an empty row range still has to raise the flags: one CTA with nothing to store
+	const int row_count = rows.y1 > rows.y0 ? rows.y1 - rows.y0 : 0;
+	const dim3 grid = row_count > 0 ? grid_for(hdr->width, row_count) : dim3(1, 1, 1), block(kBlockX, kBlockY);
+	const int pitch = history_layout->row_pitch / 8, y1 = rows.y0 + row_count;
+	cudaStream_t s = as_stream(stream);
+	if (hdr16)
+	{
+		TaaInputsT<uint2> in16{};
+		in16.hdr = view_of<const uint2>(hdr);
+		in16.depth = in.depth;
+		in16.mv = in.mv;
+		in16.history = in.history;
+#define GRB_LAUNCH16(Q, H) \
+	taa_peers_kernel<Q, H, uint2><<<grid, block, 0, s>>>(in16, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt, flag_index, epoch, scratch_counter)
+		if (!history)
+			GRB_LAUNCH16(0, false);
+		else if (quality == 0)
+			GRB_LAUNCH16(0, true);
+		else if (quality == 1)
+			GRB_LAUNCH16(1, true);
+		else
+			GRB_LAUNCH16(2, true);
+#undef GRB_LAUNCH16
+		return check_launch("grb_taa_resolve_to_peers");
+	}
+#define GRB_LAUNCH(Q, H) \
+	taa_peers_kernel<Q, H><<<grid, block, 0, s>>>(in, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt, flag_index, epoch, scratch_counter)
+	if (!history)
+		GRB_LAUNCH(0, false);
+	else if (quality == 0)
+		GRB_LAUNCH(0, true);
+	else if (quality == 1)
+		GRB_LAUNCH(1, true);
+	else
+		GRB_LAUNCH(2, true);
+#undef GRB_LAUNCH
+	return check_launch("grb_taa_resolve_to_peers");
 }
 
 // d1 .. d3 (+ temporal feedback), the average-luminance update, u2 and u1 in one cooperative launch

@@ -296,6 +296,25 @@ def taa_resolve(hdr_t, depth_t, mv_t, history_t, reproj, quality, out_color_t, o
                "grb_taa_resolve")
 
 
+def taa_resolve_to_peers(hdr_t, depth_t, mv_t, history_t, reproj, quality, out_color_t, history_images, flag_arrays, flag_index, epoch, counter_t,
+                         rows=None, own=None):
+    """grb_taa_resolve_to_peers with every rank's history image and flag array as a tensor on this device:
+    history_images[r]: (H, W, 4) uint16, flag_arrays[r]: int32 tensor; counter_t: one zeroed int32."""
+    n = len(history_images)
+    hi = _hdr_img(hdr_t)
+    oc = capi.image(out_color_t, capi.FORMAT_B10G11R11_UFLOAT)
+    layout = _img16(history_images[0])
+    di = C.byref(capi.image(depth_t, capi.FORMAT_D32_SFLOAT)) if depth_t is not None else None
+    mi = C.byref(capi.image(mv_t, capi.FORMAT_R16G16_SFLOAT)) if mv_t is not None else None
+    hs = C.byref(_img16(history_t)) if history_t is not None else None
+    rp = (C.c_float * 16)(*np.asarray(reproj, np.float32).reshape(-1).tolist()) if reproj is not None else None
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in history_images])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_taa_resolve_to_peers(C.byref(hi), di, mi, hs, rp, int(quality), C.byref(oc), C.byref(layout), images, flags, n, int(flag_index),
+                                                   int(epoch), _ptr(counter_t), capi.rows(rows), capi.rows(own), capi.stream_ptr()),
+               "grb_taa_resolve_to_peers")
+
+
 def to_dev(a):
     return _dev(a)
 

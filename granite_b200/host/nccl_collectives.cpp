@@ -88,6 +88,7 @@ NcclCollectives::~NcclCollectives()
 {
 	release_peer_exchange(bloom_d0);
 	release_peer_exchange(smaa_edge);
+	release_peer_exchange(taa_history);
 	if (comm && api().CommDestroy)
 		api().CommDestroy(comm);
 }
@@ -282,6 +283,11 @@ bool NcclCollectives::smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlo
 	return begin_frame(smaa_edge, image_bytes, slot);
 }
 
+bool NcclCollectives::taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+{
+	return begin_frame(taa_history, image_bytes, slot);
+}
+
 bool NcclCollectives::begin_frame(PeerState &peer, size_t image_bytes, PeerSlot &slot)
 {
 	if (!peer.tried || (peer.ok && peer.image_bytes != image_bytes))
@@ -291,6 +297,7 @@ bool NcclCollectives::begin_frame(PeerState &peer, size_t image_bytes, PeerSlot 
 			release_peer_exchange(peer);
 		peer.tried = true;
 		peer.ok = setup_peer_exchange(peer, image_bytes);
+		peer.epoch = 0; // the new flag arrays start at 0: a wait for the previous epoch passes on the first frame
 	}
 	if (!peer.ok)
 		return false;

@@ -30,6 +30,8 @@ public:
 	bool peer_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
 	// Second channel, same set-up and teardown: the SMAA edge rows (host/post/smaa.cpp).
 	bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
+	// Third channel: the TAA history (host/post/temporal.cpp).
+	bool taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
 
 private:
 	bool collective_failed(const char *what);
@@ -49,6 +51,7 @@ private:
 	};
 	PeerState bloom_d0;  // bloom d0 bands
 	PeerState smaa_edge; // SMAA edge rows
+	PeerState taa_history; // TAA history rows
 	bool begin_frame(PeerState &channel, size_t image_bytes, PeerSlot &slot);
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);

@@ -4,6 +4,8 @@
 #include "temporal.hpp"
 
 #include <cstring>
+#include <memory>
+#include <vector>
 
 namespace Granite
 {
@@ -118,13 +120,15 @@ void setup_taa_resolve(RenderGraph &graph, TemporalJitter &jitter, float scaling
 	auto &input_depth_res = resolve.add_texture_input(input_depth);
 	auto &history = resolve.add_history_input(output + "-history");
 
-	resolve.set_build_render_pass([&graph, &jitter, &out_color, &out_history, &input_res, &input_res_mv, &input_depth_res, &history,
+	// the history exchange of row-sharded frames: this frame's slot, and the last frame's, which holds the history
+	struct HistoryExchange
+	{
+		bool peer_stores = false;
+		RenderGraphCollectives::PeerSlot slot;
+	};
+	auto exchange = std::make_shared<HistoryExchange>();
+	resolve.set_build_render_pass([&graph, &jitter, &out_color, &out_history, &input_res, &input_res_mv, &input_depth_res, &history, exchange,
 	                               q = int(quality)](Vulkan::CommandBuffer &cmd) {
-		if (graph.is_sharded() && graph.get_shard_count() > 1)
-		{
-			Vulkan::log_error("taa-resolve: row-sharded frames are not supported (history rows would need a halo exchange).\n");
-			return;
-		}
 		GrbImage image = graph.get_physical_texture_resource(input_res).as_grb();
 		GrbImage image_mv = graph.get_physical_texture_resource(input_res_mv).as_grb();
 		GrbImage depth = graph.get_physical_texture_resource(input_depth_res).as_grb();
@@ -133,14 +137,48 @@ void setup_taa_resolve(RenderGraph &graph, TemporalJitter &jitter, float scaling
 		if (prev)
 			prev_img = prev->as_grb();
 		GrbImage oc = graph.get_physical_texture_resource(out_color).as_grb();
-		GrbImage oh = graph.get_physical_texture_resource(out_history).as_grb();
+		auto &history_view = graph.get_physical_texture_resource(out_history);
+		GrbImage oh = history_view.as_grb();
 
 		// temporal.cpp:239-243: clip(now) -> UV(previous frame)
 		mat4 reproj = translate(vec3(0.5f, 0.5f, 0.0f)) * scale(vec3(0.5f, 0.5f, 1.0f)) * jitter.get_history_view_proj(1) *
 		              jitter.get_history_inv_view_proj(0);
-		cmd.check(grb_taa_resolve(&image, &depth, &image_mv, prev ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, GrbRows{ 0, 0 },
-		                          cmd.get_stream_handle()),
-		          "grb_taa_resolve");
+		void *stream = cmd.get_stream_handle();
+		if (!(graph.is_sharded() && graph.get_shard_count() > 1))
+		{
+			cmd.check(grb_taa_resolve(&image, &depth, &image_mv, prev ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, GrbRows{ 0, 0 }, stream),
+			          "grb_taa_resolve");
+			return;
+		}
+		const ShardPlan plan = graph.get_shard_plan();
+		const RenderGraphCollectives::PeerSlot last = exchange->slot;
+		const bool had_slot = exchange->peer_stores;
+		exchange->peer_stores =
+		    graph.get_collectives()->taa_history_exchange_begin_frame((size_t)oh.row_pitch * (size_t)oh.height, exchange->slot);
+		if (exchange->peer_stores)
+		{
+			// Every rank stores its own history rows into every rank's slot of this frame, and reads last frame's slot
+			// here.  The wait is for every rank's last-frame flag: its rows of the history have landed, and it has
+			// finished reading the slot this frame overwrites (DESIGN.md section 5).  It also runs on the graph's first
+			// frame, which has no history: the channel outlives a re-bake, whose last frame read that slot.
+			const auto &slot = exchange->slot;
+			const unsigned self = graph.get_shard_rank();
+			cmd.check(grb_peer_wait(slot.flags[self], (int32_t)slot.count, slot.epoch - 1u, stream), "grb_peer_wait");
+			const bool use_history = prev && had_slot;
+			if (use_history)
+				prev_img.data = last.images[self];
+			cmd.check(grb_taa_resolve_to_peers(&image, &depth, &image_mv, use_history ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, slot.images,
+			                                   slot.flags, (int32_t)slot.count, (int32_t)self, slot.epoch, slot.counter, plan.taa, plan.own, stream),
+			          "grb_taa_resolve_to_peers");
+			return;
+		}
+		// without peer memory: the TAA rows here (the exact kernel: explicit rows), then every rank's own history rows
+		// to every rank
+		cmd.check(grb_taa_resolve(&image, &depth, &image_mv, prev ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, plan.taa, stream), "grb_taa_resolve");
+		std::vector<GrbRows> bands;
+		for (unsigned r = 0; r < graph.get_shard_count(); r++)
+			bands.push_back(graph.get_shard_plan(r).own);
+		graph.get_collectives()->all_gather_rows(cmd, history_view, bands);
 	});
 }
 } // namespace Granite

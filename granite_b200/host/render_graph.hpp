@@ -78,6 +78,14 @@ public:
 		(void)slot;
 		return false;
 	}
+	// A third channel for the TAA history (host/post/temporal.cpp): every rank's slot holds the whole history image,
+	// each rank produces its own rows of it, and the next frame reads the slot this frame filled.
+	virtual bool taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+	{
+		(void)image_bytes;
+		(void)slot;
+		return false;
+	}
 };
 
 class RenderPassInterface
@@ -470,13 +478,14 @@ public:
 	// [y0, y1) owned by rank r; they must tile the frame.  Builders scale the local band per
 	// resource with shard_rows_for(); an unsharded graph returns {0,0} (= all rows).
 	// smaa_quality_downstream: the SMAA preset (0..3) after the tonemap, -1 for none (it widens the tonemap rows).
+	// taa_upstream: a TAA resolve before the post chain (it widens the lighting rows).
 	void set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives, bool fxaa_downstream = false,
-	                    int smaa_quality_downstream = -1);
+	                    int smaa_quality_downstream = -1, bool taa_upstream = false);
 	// Rows of every stage for `rank` (this rank by default); whole images when unsharded.
 	ShardPlan get_shard_plan() const { return get_shard_plan(shard_rank); }
 	ShardPlan get_shard_plan(unsigned rank) const
 	{
-		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality);
+		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality, shard_taa);
 	}
 	GrbRows shard_rows_for(unsigned resource_height, unsigned halo_rows = 0) const;
 	GrbRows shard_rows_for_rank(unsigned rank, unsigned resource_height, unsigned halo_rows = 0) const;
@@ -538,6 +547,7 @@ private:
 	unsigned shard_rank = 0;
 	bool shard_fxaa = false;
 	int shard_smaa_quality = -1;
+	bool shard_taa = false;
 	RenderGraphCollectives *collectives = nullptr;
 
 	RenderTextureResource &get_or_create_texture(const std::string &name);

@@ -91,10 +91,10 @@ struct GrbhViewer
 	int smaa_quality() const { return uses_smaa() ? config.post_aa - GRBH_AA_SMAA_LOW : -1; }
 
 	// rows of the full-resolution inputs this rank must hold: its band + the halo the bloom
-	// threshold (and FXAA through the tonemap) reaches into
+	// threshold (and FXAA through the tonemap, TAA's neighbourhood) reaches into
 	GrbRows input_rows() const
 	{
-		return compute_shard_plan((unsigned)render_width(), (unsigned)render_height(), bands, rank, uses_fxaa(), smaa_quality()).lighting;
+		return compute_shard_plan((unsigned)render_width(), (unsigned)render_height(), bands, rank, uses_fxaa(), smaa_quality(), uses_taa()).lighting;
 	}
 
 	void upload_rows(Vulkan::CommandBuffer &cmd, RenderTextureResource *res, const void *host, unsigned texel)
@@ -127,7 +127,7 @@ void GrbhViewer::bake_render_graph()
 	dim.format = VK_FORMAT_R8G8B8A8_SRGB; // headless swapchain format (application_headless.cpp:207)
 	graph.set_backbuffer_dimensions(dim);
 	if (!bands.empty())
-		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa(), smaa_quality());
+		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa(), smaa_quality(), uses_taa());
 
 	// scene.add_render_passes(graph) -> LightClusterer::add_render_passes
 	cluster.set_resolution((unsigned)config.cluster_res[0], (unsigned)config.cluster_res[1], (unsigned)config.cluster_res[2]);
@@ -678,6 +678,20 @@ extern "C" int32_t grbh_shard_plan_smaa(int32_t width, int32_t height, const Grb
 	const GrbRows all[6] = { p.smaa_blend, p.smaa_weights, p.smaa_edges, p.smaa_edge_window, p.tonemap, p.lighting };
 	for (int i = 0; i < 6; i++)
 		out6[i] = all[i];
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_shard_plan_taa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out3)
+{
+	if (width <= 0 || height <= 0 || count < 0 || (count && !bands) || !out3 || (count && (rank < 0 || rank >= count)))
+		return fail("grbh_shard_plan_taa: bad arguments");
+	GRBH_TRY
+	std::vector<GrbRows> b(bands, bands + count);
+	ShardPlan p = compute_shard_plan((unsigned)width, (unsigned)height, b, (unsigned)rank, fxaa != 0, -1, true);
+	out3[0] = p.own;
+	out3[1] = p.taa;
+	out3[2] = p.lighting;
 	return 0;
 	GRBH_CATCH
 }

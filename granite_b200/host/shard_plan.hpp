@@ -29,6 +29,17 @@
 // So a rank that owns rows [y0, y1) produces the edges of [y0, y1) only; its weight pass runs on [y0-1, y1+2) and
 // reads the edge window [y0-2s-3, y1+2s+6), which the ranks owning those rows deliver (grb_smaa_edge_detection_to_peers);
 // blend writes [y0, y1); the tonemap covers [y0-3, y1+2).  All clamped to the image (taps clamp to the edge rows).
+//
+// TAA (taa_kernel, grb_post.cu) sits between the lighting and the post chain: its colour output "HDR-resolved" is
+// what the threshold and the tonemap read, so the TAA rows are the rows the lighting pass computes without TAA (the
+// union of the tonemap rows and the threshold's HDR rows above, for the same FXAA / SMAA settings).  A TAA texel reads
+//   current   : HDR at integer offsets -1 .. +1 in x and y (exact texel fetches, clamped to the image)
+//   velocity  : depth and mv at integer offsets -1 .. +1 (the nearest-depth footprint, exact fetches)
+//   history   : last frame's history at uv - mv (or at the reprojected position when mv = 0): any row, since the
+//               motion vectors are an input -- not a halo: every rank holds the WHOLE history, assembled from every
+//               rank's own rows of the last frame (grb_taa_resolve_to_peers, or an all-gather without peer memory).
+// No fp32 coordinate takes part in the first two, so no guard row: lighting = TAA rows +-1, clamped.  Each rank
+// produces the history of its own rows only; the TAA rows outside them are computed for the colour alone.
 #pragma once
 
 #include <vector>
@@ -45,6 +56,7 @@ struct ShardPlan
 	GrbRows upsample0;  // rows of "upsample-0" (1/4)
 	GrbRows downsample0; // rows of "downsample-0" (1/4): this rank's contribution to the all-gather
 	GrbRows threshold;  // rows of "threshold" (1/2)
+	GrbRows taa;        // rows of "HDR-resolved" the TAA resolve computes (its history: the own rows)
 	GrbRows lighting;   // rows of "HDR-main" (= rows of the G-buffer that must be resident)
 	GrbRows lum_grid;   // rows of the (d3/2) luminance grid this rank samples
 	// SMAA (smaa_quality >= 0); whole images when unsharded or without SMAA
@@ -54,6 +66,8 @@ struct ShardPlan
 	GrbRows smaa_edge_window; // rows of "smaa-edge" the weight pass reads: delivered by the ranks that own them
 };
 
-// smaa_quality: SMAA preset 0..3 (Low .. Ultra) downstream of the tonemap, -1 for none.
-ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1);
+// smaa_quality: SMAA preset 0..3 (Low .. Ultra) downstream of the tonemap, -1 for none.  taa: a TAA resolve between
+// the lighting and the post chain (it widens the lighting rows).
+ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1,
+                             bool taa = false);
 } // namespace Granite

@@ -241,6 +241,18 @@ def shard_plan_smaa(width, height, bands, rank, quality) -> dict:
     return {k: (out[i].y0, out[i].y1) for i, k in enumerate(SMAA_PLAN_FIELDS)}
 
 
+TAA_PLAN_FIELDS = ("own", "taa", "lighting")
+
+
+def shard_plan_taa(width, height, bands, rank, fxaa=False) -> dict:
+    """TAA rows one rank computes (host math of granite_b200/host/shard_plan.cpp): its own rows (whose history it
+    produces), the rows it resolves, and the lighting rows the resolve's neighbourhood needs."""
+    arr = (capi.GrbRows * max(len(bands), 1))(*[capi.GrbRows(a, b) for a, b in bands])
+    out = (capi.GrbRows * 3)()
+    _check(lib().grbh_shard_plan_taa(width, height, arr, len(bands), rank, int(fxaa), out), "grbh_shard_plan_taa")
+    return {k: (out[i].y0, out[i].y1) for i, k in enumerate(TAA_PLAN_FIELDS)}
+
+
 class Viewer:
     def __init__(self, width, height, post_aa=AA_NONE, hdr_bloom=True, dynamic_exposure=True, cuda_device=0,
                  cluster_res=(128, 64, 4096), timestamps=False, stream=None, pipelined_io=False, hdr10_output=False, hdr10_max_cll=1000.0,

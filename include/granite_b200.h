@@ -406,10 +406,28 @@ int32_t grb_fsr_sharpen(const GrbImage *color, const GrbImage *out, float sharpn
 int32_t grb_fxaa(const GrbImage *in, const GrbImage *out, GrbRows rows, void *stream);
 /* K13 taa_resolve.frag; renderer/post/temporal.cpp:226-265. history NULL on the first
  * frame (REPROJECTION_HISTORY=0). quality 0..2 = TAAQuality. mv: R16G16_SFLOAT.
- * out_color: B10G11R11_UFLOAT; out_history: R16G16B16A16_SFLOAT. */
+ * out_color: B10G11R11_UFLOAT; out_history: R16G16B16A16_SFLOAT.  GRB_TAA_TILES=1 (the tile
+ * kernel, quality 2 with history) applies to whole-frame calls, rows {0, 0}, only. */
 int32_t grb_taa_resolve(const GrbImage *hdr, const GrbImage *depth, const GrbImage *mv,
                         const GrbImage *history, const float *reproj16, int32_t quality,
                         const GrbImage *out_color, const GrbImage *out_history, GrbRows rows, void *stream);
+/* grb_taa_resolve on the rows a rank of a row-sharded frame resolves, fused with the history exchange: a texel's
+ * history read can land on any row, so every rank holds the whole history.  Colour (the values of the exact
+ * grb_taa_resolve kernel; GRB_TAA_TILES does not apply) is written to out_color on [rows.y0, rows.y1).  The history
+ * texel of each row of `own` (within rows) is stored into peer_images[r] for EVERY r, this rank's own slot
+ * (peer_images[flag_index]) included; peer_images[r] is the base address, valid on this device, of rank r's history
+ * image (cudaIpc-mapped peer memory), all with history_layout's size and pitch (history_layout->data is not used).
+ * No other history is written.  Then flags[flag_index] = epoch is release-stored into the flag array of every rank;
+ * the consumer is grb_peer_wait on all peer_count flags before the next frame's resolve reads its slot as `history`.
+ * scratch_counter: one zero-initialised uint32 in local device memory.  rows / own {0, 0} = all rows.
+ * GRB_ERR_INVALID_ARGUMENT: with history, a missing depth / mv / reproj or a history that is one of the peer images;
+ * quality outside 0..2; a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, own
+ * outside rows or the image.  GRB_ERR_UNSUPPORTED_FORMAT: formats or sizes as for grb_taa_resolve, with
+ * history_layout in out_history's place.  No reference equivalent (the reference never splits a frame). */
+int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage *depth, const GrbImage *mv, const GrbImage *history, const float *reproj16,
+                                 int32_t quality, const GrbImage *out_color, const GrbImage *history_layout, void *const *peer_images,
+                                 uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter,
+                                 GrbRows rows, GrbRows own, void *stream);
 
 #ifdef __cplusplus
 }

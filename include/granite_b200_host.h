@@ -142,6 +142,10 @@ int32_t grbh_shard_plan(int32_t width, int32_t height, const GrbRows *bands, int
  * this rank produces), edge window (the rows its weight pass reads, delivered by the ranks that own them), tonemap,
  * lighting}.  Whole images when count <= 1.  Pure host math. */
 int32_t grbh_shard_plan_smaa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t quality, GrbRows *out6);
+/* The TAA rows of the same plan with a TAA resolve before the post chain (and FXAA after it when fxaa != 0): out3 =
+ * {own (the history rows this rank produces), taa (the rows it resolves: the lighting rows of the plan without TAA),
+ * lighting (taa +- 1 row)}.  Whole images when count <= 1.  Pure host math. */
+int32_t grbh_shard_plan_taa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out3);
 
 /* bake_render_graph: declares the passes, bakes, allocates attachments. */
 int32_t grbh_viewer_bake(GrbhViewer *viewer);
