@@ -74,7 +74,9 @@ bool setup_after_post_chain_upscaling(RenderGraph &graph, const std::string &inp
 		// cmd.set_unorm_texture(0, 0, view) + NearestClamp; TARGET_SRGB follows the output's format
 		GrbImage in = graph.get_physical_texture_resource(tex).as_grb_unorm();
 		GrbImage out = graph.get_physical_texture_resource(upscale_out).as_grb();
-		cmd.check(grb_fsr_upscale(&in, &out, GrbRows{ 0, 0 }, cmd.get_stream_handle()), "grb_fsr_upscale");
+		// row-sharded: the band, +-1 row for RCAS (shard_plan.hpp); the input holds the render rows those read
+		const GrbRows rows = graph.is_sharded() && graph.get_shard_count() > 1 ? graph.get_shard_plan().easu : GrbRows{ 0, 0 };
+		cmd.check(grb_fsr_upscale(&in, &out, rows, cmd.get_stream_handle()), "grb_fsr_upscale");
 	});
 
 	if (use_sharpen)
@@ -89,7 +91,8 @@ bool setup_after_post_chain_upscaling(RenderGraph &graph, const std::string &inp
 			// picks the view from the OUTPUT's format, so the input descriptor only carries the memory
 			GrbImage in = graph.get_physical_texture_resource(upscaled).as_grb();
 			GrbImage out = graph.get_physical_texture_resource(sharpen_out).as_grb();
-			cmd.check(grb_fsr_sharpen(&in, &out, 0.5f, GrbRows{ 0, 0 }, cmd.get_stream_handle()), "grb_fsr_sharpen");
+			const GrbRows rows = graph.is_sharded() && graph.get_shard_count() > 1 ? graph.get_shard_plan().own : GrbRows{ 0, 0 };
+			cmd.check(grb_fsr_sharpen(&in, &out, 0.5f, rows, cmd.get_stream_handle()), "grb_fsr_sharpen");
 		});
 	}
 	return true;

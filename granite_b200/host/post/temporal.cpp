@@ -168,16 +168,16 @@ void setup_taa_resolve(RenderGraph &graph, TemporalJitter &jitter, float scaling
 			if (use_history)
 				prev_img.data = last.images[self];
 			cmd.check(grb_taa_resolve_to_peers(&image, &depth, &image_mv, use_history ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, slot.images,
-			                                   slot.flags, (int32_t)slot.count, (int32_t)self, slot.epoch, slot.counter, plan.taa, plan.own, stream),
+			                                   slot.flags, (int32_t)slot.count, (int32_t)self, slot.epoch, slot.counter, plan.taa, plan.render_own, stream),
 			          "grb_taa_resolve_to_peers");
 			return;
 		}
-		// without peer memory: the TAA rows here (the exact kernel: explicit rows), then every rank's own history rows
-		// to every rank
+		// without peer memory: the TAA rows here (the exact kernel: explicit rows), then every rank's produced history
+		// rows (its own band, or its render rows under FSR) to every rank
 		cmd.check(grb_taa_resolve(&image, &depth, &image_mv, prev ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, plan.taa, stream), "grb_taa_resolve");
 		std::vector<GrbRows> bands;
 		for (unsigned r = 0; r < graph.get_shard_count(); r++)
-			bands.push_back(graph.get_shard_plan(r).own);
+			bands.push_back(graph.get_shard_plan(r).render_own);
 		graph.get_collectives()->all_gather_rows(cmd, history_view, bands);
 	});
 }

@@ -775,11 +775,12 @@ void RenderGraph::log()
 }
 
 void RenderGraph::set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives_, bool fxaa_downstream,
-                                 int smaa_quality_downstream, bool taa_upstream)
+                                 int smaa_quality_downstream, bool taa_upstream, ShardUpscale upscale)
 {
 	shard_fxaa = fxaa_downstream;
 	shard_smaa_quality = smaa_quality_downstream;
 	shard_taa = taa_upstream;
+	shard_upscale = upscale;
 	if (!bands.empty())
 	{
 		if (rank >= bands.size())
@@ -793,6 +794,9 @@ void RenderGraph::set_row_shards(const std::vector<GrbRows> &bands, unsigned ran
 		}
 		if (bands.size() > 1 && !collectives_)
 			throw std::logic_error("set_row_shards: more than one band needs a collectives implementation.");
+		if (bands.size() > 1 && upscale.height)
+			compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, bands, rank, fxaa_downstream, smaa_quality_downstream,
+			                   taa_upstream, upscale); // throws when a rank would produce no render rows
 	}
 	shard_bands = bands;
 	shard_rank = rank;

@@ -479,13 +479,16 @@ public:
 	// resource with shard_rows_for(); an unsharded graph returns {0,0} (= all rows).
 	// smaa_quality_downstream: the SMAA preset (0..3) after the tonemap, -1 for none (it widens the tonemap rows).
 	// taa_upstream: a TAA resolve before the post chain (it widens the lighting rows).
+	// upscale: FSR 1 after the post chain: the render size the chain runs at, and whether RCAS follows EASU (the bands
+	// stay backbuffer rows; every stage before FSR gets render rows).
 	void set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives, bool fxaa_downstream = false,
-	                    int smaa_quality_downstream = -1, bool taa_upstream = false);
+	                    int smaa_quality_downstream = -1, bool taa_upstream = false, ShardUpscale upscale = {});
 	// Rows of every stage for `rank` (this rank by default); whole images when unsharded.
 	ShardPlan get_shard_plan() const { return get_shard_plan(shard_rank); }
 	ShardPlan get_shard_plan(unsigned rank) const
 	{
-		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality, shard_taa);
+		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality, shard_taa,
+		                          shard_upscale);
 	}
 	GrbRows shard_rows_for(unsigned resource_height, unsigned halo_rows = 0) const;
 	GrbRows shard_rows_for_rank(unsigned rank, unsigned resource_height, unsigned halo_rows = 0) const;
@@ -548,6 +551,7 @@ private:
 	bool shard_fxaa = false;
 	int shard_smaa_quality = -1;
 	bool shard_taa = false;
+	ShardUpscale shard_upscale;
 	RenderGraphCollectives *collectives = nullptr;
 
 	RenderTextureResource &get_or_create_texture(const std::string &name);

@@ -90,12 +90,25 @@ struct GrbhViewer
 	bool uses_smaa() const { return config.post_aa >= GRBH_AA_SMAA_LOW && config.post_aa <= GRBH_AA_SMAA_ULTRA; }
 	int smaa_quality() const { return uses_smaa() ? config.post_aa - GRBH_AA_SMAA_LOW : -1; }
 
-	// rows of the full-resolution inputs this rank must hold: its band + the halo the bloom
-	// threshold (and FXAA through the tonemap, TAA's neighbourhood) reaches into
-	GrbRows input_rows() const
+	// FSR 1 after the post chain: the plan's render rows are rows of the render-size image
+	ShardUpscale shard_upscale() const
 	{
-		return compute_shard_plan((unsigned)render_width(), (unsigned)render_height(), bands, rank, uses_fxaa(), smaa_quality(), uses_taa()).lighting;
+		ShardUpscale up;
+		if (upscales())
+		{
+			up.width = (unsigned)render_width();
+			up.height = (unsigned)render_height();
+			up.rcas = config.resolution_scale_sharpen != 0;
+		}
+		return up;
 	}
+	ShardPlan shard_plan() const
+	{
+		return compute_shard_plan((unsigned)config.width, (unsigned)config.height, bands, rank, uses_fxaa(), smaa_quality(), uses_taa(), shard_upscale());
+	}
+	// rows of the render-resolution inputs this rank must hold: its band + the halo the bloom
+	// threshold (and FXAA through the tonemap, TAA's neighbourhood, FSR's window) reaches into
+	GrbRows input_rows() const { return shard_plan().lighting; }
 
 	void upload_rows(Vulkan::CommandBuffer &cmd, RenderTextureResource *res, const void *host, unsigned texel)
 	{
@@ -127,7 +140,7 @@ void GrbhViewer::bake_render_graph()
 	dim.format = VK_FORMAT_R8G8B8A8_SRGB; // headless swapchain format (application_headless.cpp:207)
 	graph.set_backbuffer_dimensions(dim);
 	if (!bands.empty())
-		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa(), smaa_quality(), uses_taa());
+		graph.set_row_shards(bands, rank, collectives.get(), uses_fxaa(), smaa_quality(), uses_taa(), shard_upscale());
 
 	// scene.add_render_passes(graph) -> LightClusterer::add_render_passes
 	cluster.set_resolution((unsigned)config.cluster_res[0], (unsigned)config.cluster_res[1], (unsigned)config.cluster_res[2]);
@@ -644,9 +657,20 @@ extern "C" int32_t grbh_viewer_set_row_shards(GrbhViewer *v, const GrbRows *band
 {
 	if (!v || count < 0 || (count && !bands) || (count && (rank < 0 || rank >= count)))
 		return fail("grbh_viewer_set_row_shards: bad arguments");
-	if (count > 1 && v->upscales())
-		return fail("grbh_viewer_set_row_shards: FSR 1 upscaling (resolution_scale < 1) is not row-sharded");
 	GRBH_TRY
+	if (count > 1 && v->upscales())
+	{
+		// every rank must produce render rows for the exchanges (shard_plan.hpp)
+		try
+		{
+			compute_shard_plan((unsigned)v->config.width, (unsigned)v->config.height, std::vector<GrbRows>(bands, bands + count), (unsigned)rank,
+			                   v->uses_fxaa(), v->smaa_quality(), v->uses_taa(), v->shard_upscale());
+		}
+		catch (const std::invalid_argument &e)
+		{
+			return fail(std::string("grbh_viewer_set_row_shards: ") + e.what());
+		}
+	}
 	v->bands.assign(bands, bands + count);
 	v->rank = (unsigned)rank;
 	v->baked = false;
@@ -692,6 +716,43 @@ extern "C" int32_t grbh_shard_plan_taa(int32_t width, int32_t height, const GrbR
 	out3[0] = p.own;
 	out3[1] = p.taa;
 	out3[2] = p.lighting;
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_shard_plan_fsr(int32_t width, int32_t height, int32_t render_width, int32_t render_height, const GrbRows *bands, int32_t count,
+                                       int32_t rank, int32_t post_aa, int32_t rcas, GrbRows *out12)
+{
+	const bool known_aa = post_aa == GRBH_AA_NONE || post_aa == GRBH_AA_FXAA || (post_aa >= GRBH_AA_SMAA_LOW && post_aa <= GRBH_AA_SMAA_ULTRA) ||
+	                      (post_aa >= GRBH_AA_TAA_LOW && post_aa <= GRBH_AA_TAA_HIGH) || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	if (width <= 0 || height <= 0 || render_width <= 0 || render_height <= 0 || render_width > width || render_height > height || count < 0 ||
+	    (count && !bands) || !out12 || (count && (rank < 0 || rank >= count)) || !known_aa)
+		return fail("grbh_shard_plan_fsr: bad arguments");
+	GRBH_TRY
+	std::vector<GrbRows> b(bands, bands + count);
+	const bool fxaa = post_aa == GRBH_AA_FXAA || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	const bool taa = (post_aa >= GRBH_AA_TAA_LOW && post_aa <= GRBH_AA_TAA_HIGH) || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	const int smaa = post_aa >= GRBH_AA_SMAA_LOW && post_aa <= GRBH_AA_SMAA_ULTRA ? post_aa - GRBH_AA_SMAA_LOW : -1;
+	ShardUpscale up; // the display size itself: no upscale (the viewer runs no FSR pass then)
+	if (render_width < width || render_height < height)
+	{
+		up.width = (unsigned)render_width;
+		up.height = (unsigned)render_height;
+		up.rcas = rcas != 0;
+	}
+	ShardPlan p;
+	try
+	{
+		p = compute_shard_plan((unsigned)width, (unsigned)height, b, (unsigned)rank, fxaa, smaa, taa, up);
+	}
+	catch (const std::invalid_argument &e)
+	{
+		return fail(std::string("grbh_shard_plan_fsr: ") + e.what());
+	}
+	const GrbRows all[12] = { p.own, p.easu,     p.easu_window, p.render_own,   p.fxaa,       p.tonemap,
+		                      p.taa, p.lighting, p.smaa_blend,  p.smaa_weights, p.smaa_edges, p.smaa_edge_window };
+	for (int i = 0; i < 12; i++)
+		out12[i] = all[i];
 	return 0;
 	GRBH_CATCH
 }

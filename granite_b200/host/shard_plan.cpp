@@ -2,6 +2,8 @@
 
 #include <algorithm>
 #include <cmath>
+#include <stdexcept>
+#include <string>
 
 namespace Granite
 {
@@ -26,45 +28,113 @@ GrbRows scale_band(GrbRows band, unsigned from_h, unsigned to_h)
 	r.y1 = (int)(((uint64_t)band.y1 * to_h + from_h - 1) / from_h);
 	return r;
 }
+
+// First render row rank r produces: 8 * floor(y * Hr / (8 * Hd)) for its band's first display row y.
+int render_cut(const std::vector<GrbRows> &bands, unsigned r, unsigned height, unsigned render_height)
+{
+	if (r == 0)
+		return 0;
+	if (r >= bands.size())
+		return (int)render_height;
+	return (int)(8 * (((uint64_t)bands[r].y0 * render_height) / (8 * (uint64_t)height)));
+}
+
+// Render rows fsr_easu_kernel reads for the display rows `rows` (derivation in shard_plan.hpp).
+GrbRows easu_window(GrbRows rows, unsigned width, unsigned height, ShardUpscale up)
+{
+	float k[16];
+	grb_fsr_easu_constants((int32_t)up.width, (int32_t)up.height, (int32_t)width, (int32_t)height, k);
+	const int hr = (int)up.height;
+	auto origin = [&](float v) {
+		float f = std::floor(v * (float)hr - 0.5f);
+		f = std::fmin(std::fmax(f, -2.0f), (float)hr + 1.0f);
+		return (int)f;
+	};
+	int lo = hr, hi = -1;
+	auto add = [&](int row) {
+		row = std::min(std::max(row, 0), hr - 1);
+		lo = std::min(lo, row);
+		hi = std::max(hi, row);
+	};
+	for (int y = rows.y0; y < rows.y1; y++)
+	{
+		const float ppy = (float)y * k[1] + k[3];
+		const float fpy = std::floor(ppy);
+		const float p0y = fpy * k[5] + k[7];
+		const int o0 = origin(p0y), o1 = origin(p0y + k[9]), o2 = origin(p0y + k[11]), o3 = origin(p0y + k[13]);
+		add(o0 + 1);
+		add(o1);
+		add(o1 + 1);
+		add(o2);
+		add(o2 + 1);
+		add(o3);
+	}
+	return GrbRows{ lo, hi + 1 };
+}
 } // namespace
 
-ShardPlan compute_shard_plan(unsigned, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality, bool taa)
+ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality, bool taa,
+                             ShardUpscale upscale)
 {
 	ShardPlan p = {};
-	const GrbRows whole = { 0, (int)height };
+	const bool fsr = upscale.height > 0;
+	const unsigned hr = fsr ? upscale.height : height; // rows of every image before the FSR passes
+	const GrbRows whole = { 0, (int)hr };
 	p.smaa_blend = p.smaa_weights = p.smaa_edges = p.smaa_edge_window = whole;
-	const unsigned h_half = ceil_scale(height, 0.5f), h_quarter = ceil_scale(height, 0.25f);
-	const unsigned h_d3 = ceil_scale(height, 0.03125f), h_grid = h_d3 / 2;
+	const unsigned h_half = ceil_scale(hr, 0.5f), h_quarter = ceil_scale(hr, 0.25f);
+	const unsigned h_d3 = ceil_scale(hr, 0.03125f), h_grid = h_d3 / 2;
 	if (bands.size() <= 1)
 	{
-		GrbRows all = { 0, (int)height };
-		p.own = p.fxaa = p.tonemap = p.taa = p.lighting = all;
+		p.own = p.easu = GrbRows{ 0, (int)height };
+		p.fxaa = p.tonemap = p.taa = p.lighting = p.easu_window = p.render_own = whole;
 		p.upsample0 = p.downsample0 = GrbRows{ 0, (int)h_quarter };
 		p.threshold = GrbRows{ 0, (int)h_half };
 		p.lum_grid = GrbRows{ 0, (int)h_grid };
 		return p;
 	}
 	p.own = bands[rank];
-	p.fxaa = p.own;
-	p.tonemap = fxaa ? clamp_rows(p.own.y0 - 6, p.own.y1 + 6, height) : p.own;
+	if (fsr)
+	{
+		// derivation in shard_plan.hpp
+		for (unsigned r = 0; r < bands.size(); r++)
+			if (render_cut(bands, r + 1, height, hr) <= render_cut(bands, r, height, hr))
+				throw std::invalid_argument("FSR 1 upscaling from " + std::to_string(hr) + " to " + std::to_string(height) + " rows: rank " +
+				                            std::to_string(r) + "'s band [" + std::to_string(bands[r].y0) + ", " + std::to_string(bands[r].y1) +
+				                            ") produces no render rows (its borders fall into one 8-row unit of the render image); use wider bands");
+		p.render_own = GrbRows{ render_cut(bands, rank, height, hr), render_cut(bands, rank + 1, height, hr) };
+		p.easu = upscale.rcas ? clamp_rows(p.own.y0 - 1, p.own.y1 + 1, height) : p.own;
+		p.easu_window = easu_window(p.easu, width, height, upscale);
+	}
+	else
+		p.render_own = p.easu = p.easu_window = p.own;
+	const GrbRows fin = p.easu_window, prod = p.render_own; // final render-resolution rows, produced rows
+	p.fxaa = fin;
+	if (fsr)
+		p.fxaa.y0 &= ~15; // the FXAA tile kernel's 16-row tiles sit where they sit unsharded (shard_plan.hpp)
+	p.tonemap = fxaa ? clamp_rows(p.fxaa.y0 - 6, p.fxaa.y1 + 6, hr) : fin;
 	if (smaa_quality >= 0)
 	{
 		// derivation in shard_plan.hpp
 		const int steps = 4 << std::min(smaa_quality, 3);
-		p.smaa_blend = p.smaa_edges = p.own;
-		p.smaa_weights = clamp_rows(p.own.y0 - 1, p.own.y1 + 2, height);
-		p.smaa_edge_window = clamp_rows(p.smaa_weights.y0 - (2 * steps + 2), p.smaa_weights.y1 + 2 * steps + 4, height);
-		p.tonemap = clamp_rows(p.own.y0 - 3, p.own.y1 + 2, height);
+		p.smaa_blend = fin;
+		p.smaa_edges = prod;
+		p.smaa_weights = clamp_rows(fin.y0 - 1, fin.y1 + 2, hr);
+		p.smaa_edge_window = clamp_rows(p.smaa_weights.y0 - (2 * steps + 2), p.smaa_weights.y1 + 2 * steps + 4, hr);
+		p.tonemap = clamp_rows(std::min(fin.y0 - 2, prod.y0 - 3), std::max(fin.y1 + 2, prod.y1 + 2), hr);
 	}
 	p.upsample0 = clamp_rows(p.tonemap.y0 / 4 - 1, (p.tonemap.y1 + 3) / 4 + 1, h_quarter);
-	p.downsample0 = scale_band(p.own, height, h_quarter);
+	p.downsample0 = scale_band(prod, hr, h_quarter);
 	p.threshold = clamp_rows(2 * p.downsample0.y0 - 2, 2 * p.downsample0.y1 + 2, h_half);
-	GrbRows hdr_for_threshold = clamp_rows(2 * p.threshold.y0 - 1, 2 * p.threshold.y1 + 1, height);
-	p.taa = clamp_rows(std::min(p.tonemap.y0, hdr_for_threshold.y0), std::max(p.tonemap.y1, hdr_for_threshold.y1), height);
+	GrbRows hdr_for_threshold = clamp_rows(2 * p.threshold.y0 - 1, 2 * p.threshold.y1 + 1, hr);
+	// the TAA rows also cover the produced rows, whose history this rank pushes (without FSR the tonemap holds them)
+	p.taa = clamp_rows(std::min({ p.tonemap.y0, hdr_for_threshold.y0, prod.y0 }), std::max({ p.tonemap.y1, hdr_for_threshold.y1, prod.y1 }), hr);
 	// TAA reads HDR, depth and mv at integer offsets of +-1 row (derivation in shard_plan.hpp)
-	p.lighting = taa ? clamp_rows(p.taa.y0 - 1, p.taa.y1 + 1, height) : p.taa;
-	// luminance grid rows: row g belongs to the rank whose band holds the first backbuffer row it maps to
-	auto begin_of = [&](unsigned r) { return (int)(((uint64_t)bands[r].y0 * h_grid + height - 1) / height); };
+	p.lighting = taa ? clamp_rows(p.taa.y0 - 1, p.taa.y1 + 1, hr) : p.taa;
+	// luminance grid rows: row g belongs to the rank whose produced rows hold the first render row it maps to
+	auto begin_of = [&](unsigned r) {
+		const int y0 = fsr ? render_cut(bands, r, height, hr) : bands[r].y0;
+		return (int)(((uint64_t)y0 * h_grid + hr - 1) / hr);
+	};
 	p.lum_grid.y0 = begin_of(rank);
 	p.lum_grid.y1 = rank + 1 < bands.size() ? begin_of(rank + 1) : (int)h_grid;
 	return p;

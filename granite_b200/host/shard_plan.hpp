@@ -40,6 +40,35 @@
 //               rank's own rows of the last frame (grb_taa_resolve_to_peers, or an all-gather without peer memory).
 // No fp32 coordinate takes part in the first two, so no guard row: lighting = TAA rows +-1, clamped.  Each rank
 // produces the history of its own rows only; the TAA rows outside them are computed for the colour alone.
+//
+// FSR 1 (grb_fsr.cu) after the post chain: everything above runs at the render size (Wr x Hr), the two FSR passes
+// write the display size (Wd x Hd), and the bands are display rows.  Two row sets then differ:
+//   B (own)        the display band: what the rank owns and reads back.
+//   P (render_own) the render rows the rank PRODUCES for the exchanges (the d0 push, the SMAA edge push, the TAA
+//                  history push) and the bands of their NCCL all-gathers.  The interior boundary at display row y is
+//                  8 * floor(y * Hr / (8 * Hd)), with 0 and Hr at the two ends; every rank computes every rank's P
+//                  from the same inputs, so the ranks' P tile [0, Hr).  A layout in which some P is empty is refused.
+// Derived backwards from B:
+//   RCAS      : exact texel fetches at +-1 row (fsr_rcas_kernel)           -> RCAS rows B, EASU rows E = B +- 1
+//               (without RCAS, E = B)
+//   EASU      : output row y reads render rows around (y + 0.5) Hr / Hd - 0.5: ppy = y k1 + k3, fpy = floor(ppy),
+//               p0y = fpy k5 + k7, and four gathers at p0y, p0y + k9, p0y + k11, p0y + k13 (constants of
+//               grb_fsr_easu_constants); each gather's origin is floor(v Hr - 0.5), clamped to [-2, Hr + 1], and
+//               unorm_texel clamps the row to the edge.  Gather 0 uses only the row after its origin (b, c), gathers
+//               1 and 2 use both rows, gather 3 only its origin row (n, o).  The window W is the hull of those rows
+//               over every y in E, computed on the host with the kernel's own fp32 operations (the host library is
+//               built with -ffp-contract=off, the kernel with -fmad=false), so it is exact: no guard row.
+//   final render-resolution image (FXAA output, SMAA blend, or the tonemap without AA) -> W
+//   FXAA      : rows W with the first one rounded down to a multiple of 16, tonemap those +- 6.  The tile kernel
+//               (fxaa_fast_kernel) runs 16-row tiles from its first row and forms its bilinear coordinates in fp32
+//               relative to the tile, so a pixel's result depends on its offset in the tile: the tiles must start
+//               on the rows they start on unsharded.  Without FSR the FXAA rows stay the band, as before (a band
+//               that does not start on a multiple of 16 rows meets the same dependence there).
+//   SMAA      : blend on W, weights W-1 .. W+2, the edge window from the weights as above; edges produced on P;
+//               tonemap = hull of the blend's colour reads W-2 .. W+2 and the edge pass's P-3 .. P+2
+//   upsample0, TAA and lighting rows follow from the tonemap as above; downsample0, threshold and the luminance grid
+//   follow from P and Hr; the TAA rows also cover P, whose history the rank pushes.
+// Without FSR, W = E = P = B, and every row above is what it is without this paragraph.
 #pragma once
 
 #include <vector>
@@ -64,10 +93,23 @@ struct ShardPlan
 	GrbRows smaa_weights;     // rows of "smaa-weights" the blend reads
 	GrbRows smaa_edges;       // rows of "smaa-edge" this rank produces (= own)
 	GrbRows smaa_edge_window; // rows of "smaa-edge" the weight pass reads: delivered by the ranks that own them
+	// FSR 1 upscaling; without it easu = own and easu_window = render_own = own
+	GrbRows easu;        // display rows of the EASU output (own, +-1 with RCAS)
+	GrbRows easu_window; // render rows EASU reads for them: the rows of the final render-resolution image
+	GrbRows render_own;  // render rows this rank produces for the d0, SMAA edge and TAA history exchanges
 };
 
-// smaa_quality: SMAA preset 0..3 (Low .. Ultra) downstream of the tonemap, -1 for none.  taa: a TAA resolve between
-// the lighting and the post chain (it widens the lighting rows).
+// FSR 1 after the post chain: the render size the chain runs at (height 0: no upscale) and whether RCAS follows EASU.
+struct ShardUpscale
+{
+	unsigned width = 0, height = 0;
+	bool rcas = false;
+};
+
+// width x height: the display size the bands cut.  smaa_quality: SMAA preset 0..3 (Low .. Ultra) downstream of the
+// tonemap, -1 for none.  taa: a TAA resolve between the lighting and the post chain (it widens the lighting rows).
+// upscale: FSR 1 from the render size to the display size; throws std::invalid_argument when a rank's render rows
+// (render_own) would be empty.
 ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1,
-                             bool taa = false);
+                             bool taa = false, ShardUpscale upscale = {});
 } // namespace Granite

@@ -253,6 +253,23 @@ def shard_plan_taa(width, height, bands, rank, fxaa=False) -> dict:
     return {k: (out[i].y0, out[i].y1) for i, k in enumerate(TAA_PLAN_FIELDS)}
 
 
+FSR_PLAN_FIELDS = ("own", "easu", "easu_window", "render_own", "fxaa", "tonemap", "taa", "lighting", "smaa_blend", "smaa_weights", "smaa_edges",
+                   "smaa_edge_window")
+
+
+def shard_plan_fsr(width, height, render_width, render_height, bands, rank, post_aa=AA_NONE, rcas=True) -> dict:
+    """Rows one rank computes with FSR 1 upscaling from render_width x render_height to the display size width x height
+    (host math of granite_b200/host/shard_plan.cpp).  `bands` and `own` / `easu` are display rows: the band, and the
+    rows EASU writes (the band +- 1 with RCAS).  Everything else is render rows: `easu_window` (what EASU reads: the
+    rows of the final render-resolution image), `render_own` (what this rank produces for the exchanges), and the
+    FXAA, tonemap, TAA, lighting and SMAA rows.  post_aa: one of the AA_* codes."""
+    arr = (capi.GrbRows * max(len(bands), 1))(*[capi.GrbRows(a, b) for a, b in bands])
+    out = (capi.GrbRows * 12)()
+    _check(lib().grbh_shard_plan_fsr(width, height, render_width, render_height, arr, len(bands), rank, int(post_aa), int(rcas), out),
+           "grbh_shard_plan_fsr")
+    return {k: (out[i].y0, out[i].y1) for i, k in enumerate(FSR_PLAN_FIELDS)}
+
+
 class Viewer:
     def __init__(self, width, height, post_aa=AA_NONE, hdr_bloom=True, dynamic_exposure=True, cuda_device=0,
                  cluster_res=(128, 64, 4096), timestamps=False, stream=None, pipelined_io=False, hdr10_output=False, hdr10_max_cll=1000.0,

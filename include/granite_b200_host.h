@@ -62,7 +62,8 @@ typedef struct GrbhViewerConfig
 	float resolution_scale;          /* "resolutionScale" (scene_viewer_application.cpp:247-248): 0 or 1 = off.  < 1: width x height
 	                                  * is the DISPLAY size; the G-buffer the caller supplies (and every pass up to the post-chain
 	                                  * output) has ceil(scale * size) texels (:758-761, 888-889), and FSR 1 upscales the result
-	                                  * to the display size (:1263-1268).  Not with row sharding or HDR10 output. */
+	                                  * to the display size (:1263-1268).  Not with HDR10 output.  Row-sharded: the bands are
+	                                  * display rows; grbh_shard_plan_fsr gives the render rows each rank computes. */
 	int32_t resolution_scale_sharpen; /* "resolutionScaleSharpen" (:249-250): the RCAS pass after the upscale */
 	int32_t render_target_fp16;       /* "renderTargetFp16" (:235-236, 880-884): emissive / HDR-main are R16G16B16A16_SFLOAT (8 bytes per
 	                                   * texel -- GrbhHostGBuffer::emissive then points at RGBA16F texels); lighting, bloom threshold,
@@ -124,7 +125,8 @@ int32_t grbh_load_gtx(const char *path, int32_t *format, int32_t *width, int32_t
  * primaries_xy8: red, green, blue, white chromaticities (VkHdrMetadataEXT order); out16: column-major mat4. */
 int32_t grbh_rec709_to_display_primaries(const float *primaries_xy8, float *out16);
 
-/* Row sharding (multi-GPU): bands[r] = backbuffer rows of rank r.  Must precede bake. */
+/* Row sharding (multi-GPU): bands[r] = backbuffer rows of rank r.  Must precede bake.  With FSR 1 upscaling, a layout in
+ * which some rank would produce no render rows (grbh_shard_plan_fsr) is refused. */
 int32_t grbh_nccl_unique_id(uint8_t out128[128]);
 int32_t grbh_viewer_init_collectives(GrbhViewer *viewer, const uint8_t id128[128], int32_t rank, int32_t world_size);
 int32_t grbh_viewer_set_row_shards(GrbhViewer *viewer, const GrbRows *bands, int32_t count, int32_t rank);
@@ -146,6 +148,16 @@ int32_t grbh_shard_plan_smaa(int32_t width, int32_t height, const GrbRows *bands
  * {own (the history rows this rank produces), taa (the rows it resolves: the lighting rows of the plan without TAA),
  * lighting (taa +- 1 row)}.  Whole images when count <= 1.  Pure host math. */
 int32_t grbh_shard_plan_taa(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out3);
+/* The plan with FSR 1 upscaling after the post chain: width x height is the display size the bands cut, render_width x
+ * render_height (each 1 .. the display's) the size every pass before FSR runs at; post_aa a GrbhPostAA; rcas != 0: the
+ * sharpen pass follows the upscale.  out12 = {own (display rows), easu (the display rows EASU writes: own, +-1 row with
+ * RCAS), easu window (the render rows EASU reads: the rows of the final render-resolution image), render own (the render
+ * rows this rank produces for the exchanges), fxaa (the easu window from a multiple of 16 rows), tonemap, taa, lighting,
+ * smaa blend, smaa weights, smaa edges, smaa edge window}; everything after `easu` in render rows, the SMAA rows whole images without SMAA.  A render size equal to the
+ * display size is no upscale: the rows of grbh_shard_plan / _smaa / _taa, with easu = easu window = render own = own.
+ * Whole images when count <= 1.  Fails when some rank would produce no render rows.  Pure host math. */
+int32_t grbh_shard_plan_fsr(int32_t width, int32_t height, int32_t render_width, int32_t render_height, const GrbRows *bands, int32_t count,
+                            int32_t rank, int32_t post_aa, int32_t rcas, GrbRows *out12);
 
 /* bake_render_graph: declares the passes, bakes, allocates attachments. */
 int32_t grbh_viewer_bake(GrbhViewer *viewer);
