@@ -96,6 +96,7 @@ ENTRY_POINTS = [
     "grb_bloom_threshold", "grb_bloom_threshold_downsample", "grb_bloom_threshold_downsample_to_peers", "grb_bloom_downsample", "grb_bloom_downsample_to_peers", "grb_peer_wait", "grb_bloom_upsample", "grb_bloom_upsample_exact",
     "grb_luminance", "grb_luminance_grid", "grb_luminance_finalize", "grb_bloom_tail", "grb_bloom_tail_ex", "grb_tonemap",
     "grb_pq10_encode", "grb_smaa_edge_detection", "grb_smaa_edge_detection_to_peers", "grb_smaa_blend_weights", "grb_smaa_neighborhood_blend", "grb_fsr_easu_constants", "grb_fsr_upscale", "grb_fsr_sharpen", "grb_fxaa", "grb_taa_resolve", "grb_taa_resolve_to_peers",
+    "grb_present_rows_to_peer",
 ]
 
 _lib = None
@@ -151,6 +152,7 @@ def lib() -> C.CDLL:
             "grb_fxaa": [IMG, IMG, GrbRows, P],
             "grb_taa_resolve": [IMG, IMG, IMG, IMG, P, I, IMG, IMG, GrbRows, P],
             "grb_taa_resolve_to_peers": [IMG, IMG, IMG, IMG, P, I, IMG, IMG, P, P, I, I, C.c_uint32, P, GrbRows, GrbRows, P],
+            "grb_present_rows_to_peer": [IMG, P, P, I, I, C.c_uint32, P, GrbRows, P],
         }
         for name, args in sig.items():
             fn = getattr(_lib, name)

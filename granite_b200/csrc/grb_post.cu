@@ -194,6 +194,41 @@ __global__ void peer_wait_kernel(const uint32_t *flags, int count, uint32_t epoc
 	}
 }
 
+// Presenting a row-sharded frame from one rank: each rank copies its band of the final 4-byte-per-texel image into the
+// presenting rank's frame slot (IPC-mapped peer memory over NVLink; a local copy on the presenting rank itself), then
+// publishes "band of frame <epoch> landed" in every rank's flag array -- the protocol of bloom_downsample_peers_kernel.
+// Every rank gets the flag because the presenting rank's own flag is the credit the next frame's producers wait on.
+// One thread moves 4 texels: one 16-byte load and store when the row pitch and both bases allow it, 4-byte ones
+// otherwise and for a row's last (width mod 4) texels.  Only targets.flags is used.
+template <bool Vec16>
+__global__ void __launch_bounds__(256) present_rows_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, int pitch, int width, int y0,
+                                                          PeerTargets targets, int flag_index, uint32_t epoch, unsigned *ctas_done)
+{
+	const int x = 4 * (int)(blockIdx.x * blockDim.x + threadIdx.x);
+	if (x < width)
+	{
+		const size_t at = (size_t)(y0 + (int)blockIdx.y) * pitch + (size_t)x * 4;
+		if (Vec16 && x + 4 <= width)
+			*reinterpret_cast<uint4 *>(dst + at) = __ldg(reinterpret_cast<const uint4 *>(src + at));
+		else
+			for (int i = 0; i < 4 && x + i < width; i++)
+				reinterpret_cast<uint32_t *>(dst + at)[i] = __ldg(reinterpret_cast<const uint32_t *>(src + at) + i);
+	}
+	__threadfence_system();
+	__syncthreads();
+	if (threadIdx.x == 0)
+	{
+		const unsigned total = gridDim.x * gridDim.y;
+		if (atomicAdd(ctas_done, 1u) == total - 1u)
+		{
+			*ctas_done = 0u;
+			__threadfence_system();
+			for (int r = 0; r < targets.count; r++)
+				store_release_system(targets.flags[r] + flag_index, epoch);
+		}
+	}
+}
+
 // ------------------------------------------------------------------------------- K10
 // Average log-luminance.  The reference sums with one 8x8 workgroup: each invocation adds its
 // strided samples in (y-iter, x-iter) order, then a shared-memory tree 32,16,8,4,2 and a final
@@ -1074,6 +1109,69 @@ extern "C" int32_t grb_peer_wait(const uint32_t *local_flags, int32_t count, uin
 		max_spins = (unsigned)strtoul(e, nullptr, 10);
 	peer_wait_kernel<<<1, 32, 0, as_stream(stream)>>>(local_flags, count, epoch, device_error_word(), max_spins);
 	return check_launch("grb_peer_wait");
+}
+
+static int texel_bytes(int32_t format)
+{
+	switch (format)
+	{
+	case GRB_FORMAT_R8_UNORM: return 1;
+	case GRB_FORMAT_R8G8_UNORM: return 2;
+	case GRB_FORMAT_R16G16B16A16_SFLOAT: return 8;
+	case GRB_FORMAT_R8G8B8A8_UNORM:
+	case GRB_FORMAT_R8G8B8A8_SRGB:
+	case GRB_FORMAT_A2B10G10R10_UNORM_PACK32:
+	case GRB_FORMAT_R16G16_SFLOAT:
+	case GRB_FORMAT_B10G11R11_UFLOAT_PACK32:
+	case GRB_FORMAT_D32_SFLOAT: return 4;
+	default: return 0;
+	}
+}
+
+extern "C" int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index,
+                                            uint32_t epoch, uint32_t *scratch_counter, GrbRows own, void *stream)
+{
+	if (!src || !src->data || !dst || !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0 ||
+	    flag_index >= peer_count)
+	{
+		set_last_error("grb_present_rows_to_peer: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (texel_bytes(src->format) != 4 || src->width <= 0 || src->height <= 0 || src->row_pitch < src->width * 4 || (src->row_pitch % 4) != 0)
+	{
+		set_last_error("grb_present_rows_to_peer: src must be an image of 4-byte texels (R8G8B8A8 or A2B10G10R10)");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (dst == src->data)
+	{
+		set_last_error("grb_present_rows_to_peer: dst must be distinct from src");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (own.y0 < 0 || own.y1 <= own.y0 || own.y1 > src->height)
+	{
+		set_last_error("grb_present_rows_to_peer: own rows must be a non-empty range inside the image");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	PeerTargets targets{};
+	targets.count = peer_count;
+	for (int r = 0; r < peer_count; r++)
+	{
+		if (!peer_flags[r])
+		{
+			set_last_error("grb_present_rows_to_peer: null peer flag array");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+		targets.flags[r] = peer_flags[r];
+	}
+	const dim3 block(256), grid((unsigned)((src->width + 4 * 256 - 1) / (4 * 256)), (unsigned)(own.y1 - own.y0));
+	const auto *s = static_cast<const uint8_t *>(src->data);
+	auto *d = static_cast<uint8_t *>(dst);
+	const bool vec16 = (src->row_pitch % 16) == 0 && (reinterpret_cast<uintptr_t>(s) % 16) == 0 && (reinterpret_cast<uintptr_t>(d) % 16) == 0;
+	if (vec16)
+		present_rows_kernel<true><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets, flag_index, epoch, scratch_counter);
+	else
+		present_rows_kernel<false><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets, flag_index, epoch, scratch_counter);
+	return check_launch("grb_present_rows_to_peer");
 }
 
 static int32_t bloom_upsample_impl(const GrbImage *in, const GrbImage *out, GrbRows rows, void *stream, bool allow_tiles)

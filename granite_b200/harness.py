@@ -315,6 +315,19 @@ def taa_resolve_to_peers(hdr_t, depth_t, mv_t, history_t, reproj, quality, out_c
                "grb_taa_resolve_to_peers")
 
 
+def present_rows_to_peer(src_t, dst_t, flag_arrays, flag_index, epoch, counter_t, own, fmt=capi.FORMAT_R8G8B8A8_SRGB, width=None):
+    """grb_present_rows_to_peer with the presenting rank's slot and every rank's flag array as tensors on this device:
+    src_t / dst_t: (H, P) int32 (one 4-byte texel each; the image is the first `width` texels of each row, all P by
+    default), flag_arrays[r]: int32 tensor; counter_t: one zeroed int32."""
+    si = capi.image(src_t, fmt)
+    if width is not None:
+        si.width = int(width)
+    flags = (C.c_void_p * len(flag_arrays))(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_present_rows_to_peer(C.byref(si), dst_t.data_ptr(), flags, len(flag_arrays), int(flag_index), int(epoch),
+                                                   _ptr(counter_t), capi.rows(own), capi.stream_ptr()),
+               "grb_present_rows_to_peer")
+
+
 def to_dev(a):
     return _dev(a)
 

@@ -89,6 +89,7 @@ NcclCollectives::~NcclCollectives()
 	release_peer_exchange(bloom_d0);
 	release_peer_exchange(smaa_edge);
 	release_peer_exchange(taa_history);
+	release_peer_exchange(present);
 	if (comm && api().CommDestroy)
 		api().CommDestroy(comm);
 }
@@ -286,6 +287,11 @@ bool NcclCollectives::smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlo
 bool NcclCollectives::taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
 {
 	return begin_frame(taa_history, image_bytes, slot);
+}
+
+bool NcclCollectives::present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+{
+	return begin_frame(present, image_bytes, slot);
 }
 
 bool NcclCollectives::begin_frame(PeerState &peer, size_t image_bytes, PeerSlot &slot)

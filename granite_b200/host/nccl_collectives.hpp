@@ -32,6 +32,8 @@ public:
 	bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
 	// Third channel: the TAA history (host/post/temporal.cpp).
 	bool taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
+	// Fourth channel: the bands of the final image, pushed to the presenting rank (host/scene_viewer.cpp).
+	bool present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
 
 private:
 	bool collective_failed(const char *what);
@@ -52,6 +54,7 @@ private:
 	PeerState bloom_d0;  // bloom d0 bands
 	PeerState smaa_edge; // SMAA edge rows
 	PeerState taa_history; // TAA history rows
+	PeerState present;     // the final image on the presenting rank
 	bool begin_frame(PeerState &channel, size_t image_bytes, PeerSlot &slot);
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);

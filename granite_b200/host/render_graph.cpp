@@ -586,6 +586,13 @@ Vulkan::Stream RenderGraph::get_writer_stream(const RenderResource &resource)
 	return get_device().get_queue_stream(idx);
 }
 
+RenderGraphQueueFlagBits RenderGraph::get_writer_queue(const RenderResource &resource) const
+{
+	if (resource.get_write_passes().empty())
+		throw std::logic_error("No pass exists which writes to resource '" + resource.get_name() + "'.");
+	return passes[*std::max_element(resource.get_write_passes().begin(), resource.get_write_passes().end())]->get_queue();
+}
+
 void RenderGraph::enqueue_render_passes(Vulkan::Device &dev, TaskComposer &composer)
 {
 	if (!baked)

@@ -86,6 +86,14 @@ public:
 		(void)slot;
 		return false;
 	}
+	// A fourth channel for presenting a sharded frame from one rank (the "present" pass of scene_viewer.cpp): only the
+	// presenting rank's slots are written, each rank pushing its band of the final image into them.
+	virtual bool present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+	{
+		(void)image_bytes;
+		(void)slot;
+		return false;
+	}
 };
 
 class RenderPassInterface
@@ -471,6 +479,8 @@ public:
 	void wait_mark(const std::string &name, Vulkan::CommandBuffer &cmd);
 	// Stream of the pass that writes `resource` (for host readbacks of a graph output).
 	Vulkan::Stream get_writer_stream(const RenderResource &resource);
+	// Queue of the last declared pass that writes `resource` (before bake: where a pass that follows it belongs).
+	RenderGraphQueueFlagBits get_writer_queue(const RenderResource &resource) const;
 
 	// Execution order decided by bake(): names of the passes that will run.
 	std::vector<std::string> get_baked_pass_names() const;

@@ -58,6 +58,10 @@ struct GrbhViewer
 	std::unique_ptr<NcclCollectives> collectives;
 	std::vector<GrbRows> bands;
 	unsigned rank = 0;
+	// row-sharded frames presented from one rank (-1: off): the "present" pass gathers the bands there, and
+	// `presented` is where this frame's whole image lies on that rank (the channel's slot, or the gathered output)
+	int present_rank = -1;
+	const void *presented = nullptr;
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
@@ -109,6 +113,11 @@ struct GrbhViewer
 	// rows of the render-resolution inputs this rank must hold: its band + the halo the bloom
 	// threshold (and FXAA through the tonemap, TAA's neighbourhood, FSR's window) reaches into
 	GrbRows input_rows() const { return shard_plan().lighting; }
+	bool sharded_presenting() const { return bands.size() > 1 && present_rank >= 0; }
+
+	// the device-to-host copy of this rank's rows of the final image (the whole frame on the presenting rank), on the
+	// stream of the pass that produced it
+	cudaStream_t enqueue_readback(uint32_t *dst, GrbRows &rows);
 
 	void upload_rows(Vulkan::CommandBuffer &cmd, RenderTextureResource *res, const void *host, unsigned texel)
 	{
@@ -363,12 +372,68 @@ void GrbhViewer::bake_render_graph()
 	// scene_viewer_application.cpp:1263-1268: FSR 1 from the scaled-down image to the swapchain size
 	if (upscales() && setup_after_post_chain_upscaling(graph, ui_source, "post-scale-output", config.resolution_scale_sharpen != 0))
 		ui_source = "post-scale-output";
+	presented = nullptr;
+	if (sharded_presenting())
+	{
+		// on the stream of the pass that writes the final image, so that the readback on the presenting rank (same
+		// stream) orders its frames' pushes behind its earlier readbacks (DESIGN.md section 5, "Presenting a sharded frame")
+		auto &source = graph.get_texture_resource(ui_source);
+		auto &present = graph.add_pass("present", graph.get_writer_queue(source));
+		auto &frame = present.add_color_output("presented", source.get_attachment_info(), ui_source);
+		present.set_build_render_pass([this, &frame](Vulkan::CommandBuffer &cmd) {
+			auto &view_ = graph.get_physical_texture_resource(frame);
+			const GrbImage image = view_.as_grb();
+			void *stream = cmd.get_stream_handle();
+			const unsigned P = (unsigned)present_rank;
+			RenderGraphCollectives::PeerSlot slot;
+			if (graph.get_collectives()->present_exchange_begin_frame((size_t)image.row_pitch * (size_t)image.height, slot))
+			{
+				// the credit: P's push of the last frame ran after P's readback of the frame before, the last one that
+				// used this frame's slot
+				cmd.check(grb_peer_wait(slot.flags[rank] + P, 1, slot.epoch - 1u, stream), "grb_peer_wait");
+				cmd.check(grb_present_rows_to_peer(&image, slot.images[P], slot.flags, (int32_t)slot.count, (int32_t)rank, slot.epoch, slot.counter,
+				                                   bands[rank], stream),
+				          "grb_present_rows_to_peer");
+				if (rank == P)
+				{
+					cmd.check(grb_peer_wait(slot.flags[rank], (int32_t)slot.count, slot.epoch, stream), "grb_peer_wait");
+					presented = slot.images[P];
+				}
+				return;
+			}
+			// without peer memory: every rank's band to every rank, in place (the output image is full-size everywhere)
+			graph.get_collectives()->all_gather_rows(cmd, view_, bands);
+			presented = image.data;
+		});
+		ui_source = "presented";
+	}
 	output_name = ui_source;
 	graph.set_backbuffer_source(ui_source);
 	graph.bake();
 	// keep feed-back buffers (average luminance) across re-bakes
 	graph.install_physical_buffers(std::move(physical_buffers));
 	baked = true;
+}
+
+cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
+{
+	auto &output = graph.get_texture_resource(output_name);
+	const void *base = graph.get_physical_texture_resource(output).get_image().get_device_pointer();
+	r = bands.size() > 1 ? bands[rank] : GrbRows{ 0, config.height };
+	if (sharded_presenting() && rank == (unsigned)present_rank)
+	{
+		if (!presented)
+			throw std::runtime_error("output readback: no frame has been presented since the last bake");
+		base = presented; // the same size and pitch as the output image
+		r = GrbRows{ 0, config.height };
+	}
+	const size_t pitch = (size_t)config.width * 4;
+	auto stream = reinterpret_cast<cudaStream_t>(graph.get_writer_stream(output));
+	if (!Vulkan::cuda_ok(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(dst) + (size_t)r.y0 * pitch, static_cast<const uint8_t *>(base) + (size_t)r.y0 * pitch,
+	                                     pitch * (size_t)(r.y1 - r.y0), cudaMemcpyDeviceToHost, stream),
+	                     "output readback"))
+		throw std::runtime_error("cudaMemcpyAsync failed");
+	return stream;
 }
 
 void GrbhViewer::render_frame(const GrbhHostGBuffer *host, double frame_time)
@@ -671,11 +736,27 @@ extern "C" int32_t grbh_viewer_set_row_shards(GrbhViewer *v, const GrbRows *band
 			return fail(std::string("grbh_viewer_set_row_shards: ") + e.what());
 		}
 	}
+	if (v->present_rank >= std::max(count, 1))
+		return fail("grbh_viewer_set_row_shards: the presenting rank " + std::to_string(v->present_rank) + " would have no band among " +
+		            std::to_string(count) + " (call grbh_viewer_set_present_rank first)");
 	v->bands.assign(bands, bands + count);
 	v->rank = (unsigned)rank;
 	v->baked = false;
 	return 0;
 	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_present_rank(GrbhViewer *v, int32_t rank)
+{
+	if (!v)
+		return fail("null viewer");
+	const int32_t count = std::max((int32_t)v->bands.size(), 1); // an unsharded viewer is one band
+	if (rank < -1 || rank >= count)
+		return fail("grbh_viewer_set_present_rank: rank must be -1 (off) or within [0, " + std::to_string(count) +
+		            ") (the bands of the last grbh_viewer_set_row_shards)");
+	v->present_rank = rank;
+	v->baked = false;
+	return 0;
 }
 
 extern "C" int32_t grbh_shard_plan(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out9)
@@ -790,16 +871,8 @@ extern "C" int32_t grbh_viewer_read_output(GrbhViewer *v, uint32_t *dst, GrbRows
 	if (!v || !v->baked || !dst)
 		return fail("grbh_viewer_read_output: bad arguments");
 	GRBH_TRY
-	auto &view_ = v->graph.get_physical_texture_resource(v->graph.get_texture_resource(v->output_name));
-	GrbRows r = v->bands.size() > 1 ? v->bands[v->rank] : GrbRows{ 0, v->config.height };
-	size_t pitch = (size_t)v->config.width * 4;
-	// read back on the stream of the pass that produced the image
-	auto stream = reinterpret_cast<cudaStream_t>(v->graph.get_writer_stream(v->graph.get_texture_resource(v->output_name)));
-	auto *src = static_cast<const uint8_t *>(view_.get_image().get_device_pointer()) + (size_t)r.y0 * pitch;
-	if (!Vulkan::cuda_ok(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(dst) + (size_t)r.y0 * pitch, src, pitch * (size_t)(r.y1 - r.y0),
-	                                     cudaMemcpyDeviceToHost, stream),
-	                     "output readback"))
-		return fail("cudaMemcpyAsync failed");
+	GrbRows r;
+	cudaStream_t stream = v->enqueue_readback(dst, r);
 	if (!Vulkan::cuda_ok(cudaStreamSynchronize(stream), "cudaStreamSynchronize"))
 		return fail("cudaStreamSynchronize failed");
 	if (rows_out)
@@ -813,15 +886,8 @@ extern "C" int32_t grbh_viewer_read_output_async(GrbhViewer *v, uint32_t *dst, G
 	if (!v || !v->baked || !dst)
 		return fail("grbh_viewer_read_output_async: bad arguments");
 	GRBH_TRY
-	auto &view_ = v->graph.get_physical_texture_resource(v->graph.get_texture_resource(v->output_name));
-	GrbRows r = v->bands.size() > 1 ? v->bands[v->rank] : GrbRows{ 0, v->config.height };
-	size_t pitch = (size_t)v->config.width * 4;
-	auto stream = reinterpret_cast<cudaStream_t>(v->graph.get_writer_stream(v->graph.get_texture_resource(v->output_name)));
-	auto *src = static_cast<const uint8_t *>(view_.get_image().get_device_pointer()) + (size_t)r.y0 * pitch;
-	if (!Vulkan::cuda_ok(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(dst) + (size_t)r.y0 * pitch, src, pitch * (size_t)(r.y1 - r.y0),
-	                                     cudaMemcpyDeviceToHost, stream),
-	                     "output readback"))
-		return fail("cudaMemcpyAsync failed");
+	GrbRows r;
+	cudaStream_t stream = v->enqueue_readback(dst, r);
 	cudaEvent_t e;
 	if (!v->free_output_events.empty())
 	{

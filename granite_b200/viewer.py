@@ -377,6 +377,11 @@ class Viewer:
         arr = (capi.GrbRows * len(bands))(*[capi.GrbRows(a, b) for a, b in bands])
         _check(lib().grbh_viewer_set_row_shards(self._h, arr, len(bands), rank), "grbh_viewer_set_row_shards")
 
+    def set_present_rank(self, rank):
+        """Present row-sharded frames from `rank` (-1: off): read_output / read_output_async there return the whole
+        frame.  Every rank sets the same value, before bake."""
+        _check(lib().grbh_viewer_set_present_rank(self._h, int(rank)), "grbh_viewer_set_present_rank")
+
     def bake(self):
         _check(lib().grbh_viewer_bake(self._h), "grbh_viewer_bake")
 

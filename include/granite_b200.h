@@ -429,6 +429,19 @@ int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage *depth, con
                                  uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter,
                                  GrbRows rows, GrbRows own, void *stream);
 
+/* Presenting a row-sharded frame from one rank: copies the rows `own` of src (4-byte texels: R8G8B8A8_SRGB / _UNORM, or
+ * A2B10G10R10_UNORM_PACK32 for HDR10) into dst at the same rows.  dst is the base address, valid on this device, of the
+ * presenting rank's frame slot (cudaIpc-mapped peer memory, or local memory on the presenting rank itself) with src's
+ * size and pitch.  16-byte loads and stores where the pitch and both bases are 16-byte aligned, 4-byte ones otherwise.
+ * Then flags[flag_index] = epoch is release-stored into the flag array of EVERY rank: the presenting rank waits on all
+ * peer_count flags before it reads the slot, and every rank waits on the presenting rank's flag of the last frame (the
+ * credit) before it writes the slot again.  scratch_counter: one zero-initialised uint32 in local device memory.
+ * GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1,
+ * own empty or outside the image, a texel size other than 4 bytes, dst equal to src->data.  No reference equivalent
+ * (the reference never splits a frame). */
+int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch,
+                                 uint32_t *scratch_counter, GrbRows own, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -126,10 +126,19 @@ int32_t grbh_load_gtx(const char *path, int32_t *format, int32_t *width, int32_t
 int32_t grbh_rec709_to_display_primaries(const float *primaries_xy8, float *out16);
 
 /* Row sharding (multi-GPU): bands[r] = backbuffer rows of rank r.  Must precede bake.  With FSR 1 upscaling, a layout in
- * which some rank would produce no render rows (grbh_shard_plan_fsr) is refused. */
+ * which some rank would produce no render rows (grbh_shard_plan_fsr) is refused, and so is a layout with fewer bands
+ * than the presenting rank of grbh_viewer_set_present_rank needs. */
 int32_t grbh_nccl_unique_id(uint8_t out128[128]);
 int32_t grbh_viewer_init_collectives(GrbhViewer *viewer, const uint8_t id128[128], int32_t rank, int32_t world_size);
 int32_t grbh_viewer_set_row_shards(GrbhViewer *viewer, const GrbRows *bands, int32_t count, int32_t rank);
+/* Presents row-sharded frames from one rank (the one that owns the swapchain): a "present" pass at the end of every
+ * frame pushes each rank's band of the final image into that rank's memory (NVLink peer stores, or an NCCL all-gather
+ * without peer memory), and grbh_viewer_read_output / _async on that rank return the whole frame, rows {0, height}.
+ * Other ranks still return their bands.  rank: -1 = off (the default), otherwise within [0, band count) of the last
+ * grbh_viewer_set_row_shards; an unsharded viewer counts as one band, so 0 is accepted there and changes nothing.
+ * Every rank must set the same value.  Must precede bake.  Readers of the presented frame must be stream-ordered
+ * behind the frame (these readbacks are): DESIGN.md section 5, "Presenting a sharded frame". */
+int32_t grbh_viewer_set_present_rank(GrbhViewer *viewer, int32_t rank);
 
 /* Work estimate of the lighting pass per group of 4 backbuffer rows for the frame last rendered by
  * an UNSHARDED viewer (its depth image and light cluster are resident): grb_lighting_row_cost() on
@@ -166,7 +175,8 @@ int32_t grbh_viewer_bake(GrbhViewer *viewer);
  * pass on the stream.  Asynchronous; ordering with later calls is stream order. */
 int32_t grbh_viewer_render_frame(GrbhViewer *viewer, const GrbhHostGBuffer *host_gbuffer, double frame_time);
 /* Copies this rank's rows of the final image (R8G8B8A8) to host memory laid out as the full
- * frame (row pitch = width*4) and waits for it. rows_out receives the band. */
+ * frame (row pitch = width*4) and waits for it. rows_out receives the band (the whole frame on
+ * the presenting rank, grbh_viewer_set_present_rank). */
 int32_t grbh_viewer_read_output(GrbhViewer *viewer, uint32_t *dst_full_frame, GrbRows *rows_out);
 /* Asynchronous form: enqueues the device->host copy of this frame's rows behind the frame and
  * returns; grbh_viewer_wait_outputs(viewer, k) blocks until at most k such copies are pending
