@@ -180,6 +180,12 @@ def bloom_upsample(in_t, out_t, rows=None):
     capi.check(capi.lib().grb_bloom_upsample(C.byref(ii), C.byref(oi), capi.rows(rows), capi.stream_ptr()), "grb_bloom_upsample")
 
 
+def bloom_upsample_exact(in_t, out_t, rows=None):
+    """The shader's arithmetic at every size (no tile kernel): the u0 a frame computes when the fused tail does not run."""
+    ii, oi = _img16(in_t), _img16(out_t)
+    capi.check(capi.lib().grb_bloom_upsample_exact(C.byref(ii), C.byref(oi), capi.rows(rows), capi.stream_ptr()), "grb_bloom_upsample_exact")
+
+
 def bloom_tail(d0_t, d1_t, d2_t, d3_t, history_t, lerp_d3, lum_t, lerp_lum, u2_t, u1_t, lo=-3.0, hi=2.0, u0_t=None, u0_rows=None, max_ctas=0):
     """d1, d2, d3 (+feedback), luminance, u2, u1 in one cooperative launch; with u0_t also (rows of) u0."""
     im = [_img16(t) for t in (d0_t, d1_t, d2_t, d3_t, u2_t, u1_t)]

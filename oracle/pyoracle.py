@@ -506,16 +506,17 @@ def luminance(d3, lum3, lerp, lo=-3.0, hi=2.0, want_grid=False):
     return (l3, grid) if want_grid else l3
 
 
-def tonemap(hdr, bloom, lum3, exposure=1.0, rows=None):
+def tonemap(hdr, bloom, lum3, exposure=1.0, rows=None, target_srgb=True):
+    """target_srgb: an R8G8B8A8_SRGB attachment (the swapchain) or, when False, the UNORM store of the linear value."""
     h, w = hdr.shape[:2]
     bh, bw = bloom.shape[:2]
     out = np.zeros((h, w), np.uint32)
     l3 = None if lum3 is None else _c(lum3, np.float32)
     y0, y1 = rows if rows else (0, h)
     if hdr.ndim == 3:
-        lib().orc_tonemap_fp16(_p(_c(hdr, np.uint16)), w, h, _p(_c(bloom, np.uint16)), bw, bh, _p(l3), _f(exposure), _p(out), y0, y1)
+        lib().orc_tonemap_fp16(_p(_c(hdr, np.uint16)), w, h, _p(_c(bloom, np.uint16)), bw, bh, _p(l3), _f(exposure), int(target_srgb), _p(out), y0, y1)
     else:
-        lib().orc_tonemap(_p(_c(hdr, np.uint32)), w, h, _p(_c(bloom, np.uint16)), bw, bh, _p(l3), _f(exposure), _p(out), y0, y1)
+        lib().orc_tonemap(_p(_c(hdr, np.uint32)), w, h, _p(_c(bloom, np.uint16)), bw, bh, _p(l3), _f(exposure), int(target_srgb), _p(out), y0, y1)
     return out
 
 
