@@ -8,6 +8,7 @@
 // rows of one screen-row shard), reading packed texels straight from HBM/L2 with 4/8-byte
 // coalesced accesses; the small pyramid levels live entirely in the 50 MB L2.
 #include "grb_common.cuh"
+#include "grb_peer.cuh"
 
 #include <cooperative_groups.h>
 
@@ -122,26 +123,10 @@ __global__ void __launch_bounds__(kBlockX *kBlockY) bloom_upsample_kernel(View<c
 // to a collective afterwards, the kernel stores each texel straight into the 1/4-resolution image
 // of every rank (its own and the peers' over NVLink / NVSwitch, plain 8-byte stores to mapped
 // peer memory) and then publishes "band of frame <epoch> landed" in every rank's flag array.
-// The consumer side is peer_wait_kernel below.  Texel values are those of
-// bloom_downsample_kernel<false>.
-struct PeerTargets
-{
-	uint2 *data[GRB_MAX_PEERS];
-	uint32_t *flags[GRB_MAX_PEERS];
-	int count;
-};
-
-__device__ __forceinline__ void store_release_system(uint32_t *p, uint32_t v) { asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-__device__ __forceinline__ uint32_t load_acquire_system(const uint32_t *p)
-{
-	uint32_t v;
-	asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-	return v;
-}
-
+// The consumer side is peer_wait_kernel below; the protocol is grb_peer.cuh's.  Texel values are
+// those of bloom_downsample_kernel<false>.
 __global__ void __launch_bounds__(kBlockX *kBlockY) bloom_downsample_peers_kernel(View<const uint2> src, PeerTargets targets, int out_w, int out_pitch_texels,
-                                                                                 int y0, int y1, float inv_w, float inv_h, float inv_in_w, float inv_in_h,
-                                                                                 int flag_index, uint32_t epoch, unsigned *ctas_done)
+                                                                                 int y0, int y1, float inv_w, float inv_h, float inv_in_w, float inv_in_h)
 {
 	const int x = blockIdx.x * kBlockX + threadIdx.x;
 	const int y = y0 + blockIdx.y * kBlockY + threadIdx.y;
@@ -152,58 +137,29 @@ __global__ void __launch_bounds__(kBlockX *kBlockY) bloom_downsample_peers_kerne
 		const uint2 texel = pack_rgba16f(tent9(src, u, v, 1.75f, inv_in_w, inv_in_h));
 		const size_t at = (size_t)y * out_pitch_texels + x;
 		for (int r = 0; r < targets.count; r++)
-			targets.data[r][at] = texel;
+			static_cast<uint2 *>(targets.data[r])[at] = texel;
 	}
-	// publish: every thread's stores are ordered before its CTA's arrival; the last CTA to arrive
-	// raises this rank's flag on every peer (threadFenceReduction pattern at system scope)
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0 && threadIdx.y == 0)
-	{
-		const unsigned total = gridDim.x * gridDim.y;
-		if (atomicAdd(ctas_done, 1u) == total - 1u)
-		{
-			*ctas_done = 0u;
-			__threadfence_system();
-			for (int r = 0; r < targets.count; r++)
-				store_release_system(targets.flags[r] + flag_index, epoch);
-		}
-	}
+	peer_publish(targets);
 }
 
 // One thread per producing rank spins until that rank's band of frame `epoch` has landed here.
 __global__ void peer_wait_kernel(const uint32_t *flags, int count, uint32_t epoch, uint32_t *error_word, unsigned max_spins)
 {
 	if ((int)threadIdx.x < count)
-	{
-		// bounded (~4 s): a rank that died must not hang the GPUs of the others
-		for (unsigned spins = 0; (int32_t)(load_acquire_system(flags + threadIdx.x) - epoch) < 0; spins++)
-		{
-			if (spins > max_spins)
-			{
-				printf("granite_b200: timed out waiting for rank %d's band of frame %u\n", (int)threadIdx.x, epoch);
-				if (error_word) // picked up by the next grb_* call on this device (check_launch)
-				{
-					*reinterpret_cast<volatile uint32_t *>(error_word) = (GRB_DEVICE_ERROR_PEER_TIMEOUT << 24) | ((uint32_t)threadIdx.x << 16) | (epoch & 0xffffu);
-					__threadfence_system();
-				}
-				break;
-			}
-			__nanosleep(128);
-		}
-	}
+		peer_wait(flags, threadIdx.x, epoch, error_word, max_spins);
 }
 
 // Presenting a row-sharded frame from one rank: each rank copies its band of the final 4-byte-per-texel image into the
 // presenting rank's frame slot (IPC-mapped peer memory over NVLink; a local copy on the presenting rank itself), then
-// publishes "band of frame <epoch> landed" in every rank's flag array -- the protocol of bloom_downsample_peers_kernel.
+// publishes "band of frame <epoch> landed" in every rank's flag array (grb_peer.cuh).
 // Every rank gets the flag because the presenting rank's own flag is the credit the next frame's producers wait on.
 // One thread moves 4 texels: one 16-byte load and store when the row pitch and both bases allow it, 4-byte ones
 // otherwise and for a row's last (width mod 4) texels.  Only targets.flags is used.
 template <bool Vec16>
 __global__ void __launch_bounds__(256) present_rows_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst, int pitch, int width, int y0,
-                                                          PeerTargets targets, int flag_index, uint32_t epoch, unsigned *ctas_done)
+                                                          PeerTargets targets)
 {
+	__builtin_assume(threadIdx.y == 0); // 1-D blocks: peer_publish's leader test is threadIdx.x == 0
 	const int x = 4 * (int)(blockIdx.x * blockDim.x + threadIdx.x);
 	if (x < width)
 	{
@@ -214,19 +170,7 @@ __global__ void __launch_bounds__(256) present_rows_kernel(const uint8_t *__rest
 			for (int i = 0; i < 4 && x + i < width; i++)
 				reinterpret_cast<uint32_t *>(dst + at)[i] = __ldg(reinterpret_cast<const uint32_t *>(src + at) + i);
 	}
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0)
-	{
-		const unsigned total = gridDim.x * gridDim.y;
-		if (atomicAdd(ctas_done, 1u) == total - 1u)
-		{
-			*ctas_done = 0u;
-			__threadfence_system();
-			for (int r = 0; r < targets.count; r++)
-				store_release_system(targets.flags[r] + flag_index, epoch);
-		}
-	}
+	peer_publish(targets);
 }
 
 // ------------------------------------------------------------------------------- K10
@@ -784,12 +728,11 @@ __global__ void __launch_bounds__(kBlockX *kBlockY) taa_kernel(TaaInputsT<HdrTex
 // Row-sharded frames: a texel's history read (at uv - mv) can land on any row, so every rank needs the whole history
 // of the last frame.  Each rank resolves its TAA rows [y0, y1) (colour into its own image) and stores the history of
 // its own rows [own0, own1) into the history slot of every rank, its own included (plain 8-byte stores to IPC-mapped
-// peer memory over NVLink), then publishes "history rows of frame <epoch> landed" in every rank's flag array -- the
-// protocol of bloom_downsample_peers_kernel.  The consumer side is grb_peer_wait before the next frame's resolve.
+// peer memory over NVLink), then publishes "history rows of frame <epoch> landed" in every rank's flag array
+// (grb_peer.cuh).  The consumer side is grb_peer_wait before the next frame's resolve.
 template <int Quality, bool History, typename HdrTexel = uint32_t>
 __global__ void __launch_bounds__(kBlockX *kBlockY) taa_peers_kernel(TaaInputsT<HdrTexel> in, Mat4 reproj, View<uint32_t> out_color, PeerTargets targets,
-                                                                    int pitch_texels, int y0, int y1, int own0, int own1, float4 rt, int flag_index,
-                                                                    uint32_t epoch, unsigned *ctas_done)
+                                                                    int pitch_texels, int y0, int y1, int own0, int own1, float4 rt)
 {
 	const int x = blockIdx.x * kBlockX + threadIdx.x;
 	const int y = y0 + blockIdx.y * kBlockY + threadIdx.y;
@@ -801,24 +744,12 @@ __global__ void __launch_bounds__(kBlockX *kBlockY) taa_peers_kernel(TaaInputsT<
 		{
 			const size_t at = (size_t)y * pitch_texels + x;
 			for (int r = 0; r < targets.count; r++)
-				targets.data[r][at] = t.history;
+				static_cast<uint2 *>(targets.data[r])[at] = t.history;
 		}
 	}
-	// as bloom_downsample_peers_kernel: the last CTA to arrive raises this rank's flag on every rank.  Each CTA's history
-	// reads are done before it arrives, so the flag also says "this rank has finished reading last frame's slot".
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0 && threadIdx.y == 0)
-	{
-		const unsigned total = gridDim.x * gridDim.y;
-		if (atomicAdd(ctas_done, 1u) == total - 1u)
-		{
-			*ctas_done = 0u;
-			__threadfence_system();
-			for (int r = 0; r < targets.count; r++)
-				store_release_system(targets.flags[r] + flag_index, epoch);
-		}
-	}
+	// Each CTA's history reads are done before it arrives, so the flag also says "this rank has finished reading last
+	// frame's slot".
+	peer_publish(targets);
 }
 
 // ------------------------------------------------------------------------------- pyramid tail
@@ -920,21 +851,7 @@ __global__ void __launch_bounds__(kTailThreads) bloom_tail_kernel(const TailArgs
 		// fills the machine; they are few (max_ctas) and spin with nanosleep.  Bounded (~4 s): a rank that
 		// died must not hang the GPUs of the others.
 		if ((int)threadIdx.x < a.wait_count)
-			for (unsigned spins = 0; (int32_t)(load_acquire_system(a.wait_flags + threadIdx.x) - a.wait_epoch) < 0; spins++)
-			{
-				if (spins > a.max_spins)
-				{
-					if (blockIdx.x == 0)
-						printf("granite_b200: timed out waiting for rank %d's band of frame %u\n", (int)threadIdx.x, a.wait_epoch);
-					if (a.error_word) // picked up by the next grb_* call on this device (check_launch)
-					{
-						*reinterpret_cast<volatile uint32_t *>(a.error_word) = (GRB_DEVICE_ERROR_PEER_TIMEOUT << 24) | ((uint32_t)threadIdx.x << 16) | (a.wait_epoch & 0xffffu);
-						__threadfence_system();
-					}
-					break;
-				}
-				__nanosleep(128);
-			}
+			peer_wait(a.wait_flags, threadIdx.x, a.wait_epoch, a.error_word, a.max_spins);
 		__syncthreads();
 	}
 	tail_level(a.d0, a.d1, 1.75f, nullptr, 0.0f, 0u, gridDim.x);
@@ -1065,34 +982,20 @@ extern "C" int32_t grb_bloom_downsample_to_peers(const GrbImage *in, const GrbIm
                                                  int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, GrbRows rows,
                                                  void *stream)
 {
-	if (!image_ok(in, GRB_FORMAT_R16G16B16A16_SFLOAT, 8) || !out_layout || out_layout->format != GRB_FORMAT_R16G16B16A16_SFLOAT || !peer_images ||
-	    !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0 || (out_layout->row_pitch % 8) != 0)
+	if (!image_ok(in, GRB_FORMAT_R16G16B16A16_SFLOAT, 8) || !out_layout || out_layout->format != GRB_FORMAT_R16G16B16A16_SFLOAT ||
+	    (out_layout->row_pitch % 8) != 0)
 	{
 		set_last_error("grb_bloom_downsample_to_peers: bad arguments");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	PeerTargets targets;
+	if (!peer_targets_from("grb_bloom_downsample_to_peers", peer_images, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
+		return GRB_ERR_INVALID_ARGUMENT;
 	rows = full_rows(rows, out_layout->height);
-	PeerTargets targets{};
-	targets.count = peer_count;
-	for (int r = 0; r < peer_count; r++)
-	{
-		if (!peer_images[r] || !peer_flags[r])
-		{
-			set_last_error("grb_bloom_downsample_to_peers: null peer pointer");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
-		targets.data[r] = static_cast<uint2 *>(peer_images[r]);
-		targets.flags[r] = peer_flags[r];
-	}
-	// an empty band still has to raise the flags: one CTA with nothing to store
 	const int row_count = rows.y1 > rows.y0 ? rows.y1 - rows.y0 : 0;
-	dim3 grid = grid_for(out_layout->width, row_count > 0 ? row_count : 1), block(kBlockX, kBlockY);
-	if (row_count == 0)
-		grid = dim3(1, 1, 1);
-	bloom_downsample_peers_kernel<<<grid, block, 0, as_stream(stream)>>>(
+	bloom_downsample_peers_kernel<<<peer_grid(row_count, grid_for(out_layout->width, row_count)), dim3(kBlockX, kBlockY), 0, as_stream(stream)>>>(
 	    view_of<const uint2>(in), targets, row_count > 0 ? out_layout->width : 0, out_layout->row_pitch / 8, rows.y0, rows.y0 + row_count,
-	    1.0f / (float)out_layout->width, 1.0f / (float)out_layout->height, 1.0f / (float)in->width, 1.0f / (float)in->height, flag_index, epoch,
-	    scratch_counter);
+	    1.0f / (float)out_layout->width, 1.0f / (float)out_layout->height, 1.0f / (float)in->width, 1.0f / (float)in->height);
 	return check_launch("grb_bloom_downsample_to_peers");
 }
 
@@ -1103,11 +1006,7 @@ extern "C" int32_t grb_peer_wait(const uint32_t *local_flags, int32_t count, uin
 		set_last_error("grb_peer_wait: bad arguments");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	// ~4 s by default; GRB_PEER_WAIT_SPINS shortens the bound (tests of the timeout path)
-	unsigned max_spins = 1u << 25;
-	if (const char *e = getenv("GRB_PEER_WAIT_SPINS"))
-		max_spins = (unsigned)strtoul(e, nullptr, 10);
-	peer_wait_kernel<<<1, 32, 0, as_stream(stream)>>>(local_flags, count, epoch, device_error_word(), max_spins);
+	peer_wait_kernel<<<1, 32, 0, as_stream(stream)>>>(local_flags, count, epoch, device_error_word(), peer_wait_max_spins());
 	return check_launch("grb_peer_wait");
 }
 
@@ -1131,12 +1030,14 @@ static int texel_bytes(int32_t format)
 extern "C" int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index,
                                             uint32_t epoch, uint32_t *scratch_counter, GrbRows own, void *stream)
 {
-	if (!src || !src->data || !dst || !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0 ||
-	    flag_index >= peer_count)
+	if (!src || !src->data || !dst)
 	{
-		set_last_error("grb_present_rows_to_peer: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1");
+		set_last_error("grb_present_rows_to_peer: null pointer");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	PeerTargets targets;
+	if (!peer_targets_from("grb_present_rows_to_peer", nullptr, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets, true))
+		return GRB_ERR_INVALID_ARGUMENT;
 	if (texel_bytes(src->format) != 4 || src->width <= 0 || src->height <= 0 || src->row_pitch < src->width * 4 || (src->row_pitch % 4) != 0)
 	{
 		set_last_error("grb_present_rows_to_peer: src must be an image of 4-byte texels (R8G8B8A8 or A2B10G10R10)");
@@ -1152,25 +1053,14 @@ extern "C" int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint
 		set_last_error("grb_present_rows_to_peer: own rows must be a non-empty range inside the image");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	PeerTargets targets{};
-	targets.count = peer_count;
-	for (int r = 0; r < peer_count; r++)
-	{
-		if (!peer_flags[r])
-		{
-			set_last_error("grb_present_rows_to_peer: null peer flag array");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
-		targets.flags[r] = peer_flags[r];
-	}
 	const dim3 block(256), grid((unsigned)((src->width + 4 * 256 - 1) / (4 * 256)), (unsigned)(own.y1 - own.y0));
 	const auto *s = static_cast<const uint8_t *>(src->data);
 	auto *d = static_cast<uint8_t *>(dst);
 	const bool vec16 = (src->row_pitch % 16) == 0 && (reinterpret_cast<uintptr_t>(s) % 16) == 0 && (reinterpret_cast<uintptr_t>(d) % 16) == 0;
 	if (vec16)
-		present_rows_kernel<true><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets, flag_index, epoch, scratch_counter);
+		present_rows_kernel<true><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets);
 	else
-		present_rows_kernel<false><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets, flag_index, epoch, scratch_counter);
+		present_rows_kernel<false><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets);
 	return check_launch("grb_present_rows_to_peer");
 }
 
@@ -1451,28 +1341,15 @@ extern "C" int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage 
 		set_last_error("grb_taa_resolve_to_peers: quality must be 0..2");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	if (!peer_images || !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0 || flag_index >= peer_count)
-	{
-		set_last_error("grb_taa_resolve_to_peers: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1");
+	PeerTargets targets;
+	if (!peer_targets_from("grb_taa_resolve_to_peers", peer_images, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
 		return GRB_ERR_INVALID_ARGUMENT;
-	}
-	PeerTargets targets{};
-	targets.count = peer_count;
 	for (int r = 0; r < peer_count; r++)
-	{
-		if (!peer_images[r] || !peer_flags[r])
-		{
-			set_last_error("grb_taa_resolve_to_peers: null peer pointer");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
 		if (history && history->data == peer_images[r])
 		{
 			set_last_error("grb_taa_resolve_to_peers: the history input must be distinct from every peer image");
 			return GRB_ERR_INVALID_ARGUMENT;
 		}
-		targets.data[r] = static_cast<uint2 *>(peer_images[r]);
-		targets.flags[r] = peer_flags[r];
-	}
 	rows = full_rows(rows, hdr->height);
 	if (own.y0 == 0 && own.y1 == 0)
 		own.y1 = hdr->height;
@@ -1494,9 +1371,8 @@ extern "C" int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage 
 	}
 	auto oc = view_of<uint32_t>(out_color);
 	float4 rt = make_float4(1.0f / (float)hdr->width, 1.0f / (float)hdr->height, (float)hdr->width, (float)hdr->height);
-	// an empty row range still has to raise the flags: one CTA with nothing to store
 	const int row_count = rows.y1 > rows.y0 ? rows.y1 - rows.y0 : 0;
-	const dim3 grid = row_count > 0 ? grid_for(hdr->width, row_count) : dim3(1, 1, 1), block(kBlockX, kBlockY);
+	const dim3 grid = peer_grid(row_count, grid_for(hdr->width, row_count)), block(kBlockX, kBlockY);
 	const int pitch = history_layout->row_pitch / 8, y1 = rows.y0 + row_count;
 	cudaStream_t s = as_stream(stream);
 	if (hdr16)
@@ -1507,7 +1383,7 @@ extern "C" int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage 
 		in16.mv = in.mv;
 		in16.history = in.history;
 #define GRB_LAUNCH16(Q, H) \
-	taa_peers_kernel<Q, H, uint2><<<grid, block, 0, s>>>(in16, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt, flag_index, epoch, scratch_counter)
+	taa_peers_kernel<Q, H, uint2><<<grid, block, 0, s>>>(in16, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt)
 		if (!history)
 			GRB_LAUNCH16(0, false);
 		else if (quality == 0)
@@ -1520,7 +1396,7 @@ extern "C" int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage 
 		return check_launch("grb_taa_resolve_to_peers");
 	}
 #define GRB_LAUNCH(Q, H) \
-	taa_peers_kernel<Q, H><<<grid, block, 0, s>>>(in, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt, flag_index, epoch, scratch_counter)
+	taa_peers_kernel<Q, H><<<grid, block, 0, s>>>(in, m, oc, targets, pitch, rows.y0, y1, own.y0, own.y1, rt)
 	if (!history)
 		GRB_LAUNCH(0, false);
 	else if (quality == 0)
@@ -1632,8 +1508,7 @@ extern "C" int32_t grb_bloom_tail_ex(const GrbImage *d0, const GrbImage *d1, con
 			a.wait_count = opt->peer_count;
 			a.wait_epoch = opt->peer_epoch;
 			a.error_word = device_error_word();
-			if (const char *e = getenv("GRB_PEER_WAIT_SPINS"))
-				a.max_spins = (unsigned)strtoul(e, nullptr, 10);
+			a.max_spins = peer_wait_max_spins();
 		}
 		max_ctas = opt->max_ctas;
 	}

@@ -29,6 +29,7 @@
 // configurations (4K: 3840 -> 1920 -> 960 -> 480 -> 240; only 240x135 -> 120x68 and back are not
 // 2:1 and stay on the generic path, 0.3 MB).
 #include "grb_common.cuh"
+#include "grb_peer.cuh"
 
 #include <cuda.h>
 
@@ -273,17 +274,8 @@ __global__ void __launch_bounds__(kThreads) tent_tile_kernel(const __grid_consta
 
 // ---------------------------------------------------------------------------------- K7 + K8 fused
 // Row-sharded frames: the d0 band is stored into the 1/4-resolution image of EVERY rank (peer memory over
-// NVLink / NVSwitch) and the last CTA publishes the frame's epoch in every rank's flag array -- the
-// protocol of bloom_downsample_peers_kernel in grb_post.cu, see there.
-struct HeadPeers
-{
-	uint2 *data[GRB_MAX_PEERS];
-	uint32_t *flags[GRB_MAX_PEERS];
-	int count; // 0: plain local store to HeadArgs::d0
-	int flag_index;
-	uint32_t epoch;
-	unsigned *ctas_done;
-};
+// NVLink / NVSwitch) and the last CTA publishes the frame's epoch in every rank's flag array
+// (grb_peer.cuh).  peers.count == 0: plain local store to HeadArgs::d0.
 
 struct HeadArgs
 {
@@ -304,8 +296,9 @@ struct AxisRec
 };
 
 template <bool DynamicExposure>
-__global__ void __launch_bounds__(kThreads) bloom_head_kernel(const __grid_constant__ CUtensorMap hdr_map, const HeadArgs a, const HeadPeers peers)
+__global__ void __launch_bounds__(kThreads) bloom_head_kernel(const __grid_constant__ CUtensorMap hdr_map, const HeadArgs a, const PeerTargets peers)
 {
+	__builtin_assume(threadIdx.y == 0); // 1-D blocks: peer_publish's leader test is threadIdx.x == 0
 	extern __shared__ __align__(128) unsigned char smem[];
 	uint32_t *hdr = reinterpret_cast<uint32_t *>(smem);                                    // 136 x 72 B10G11R11
 	float4 *tile = reinterpret_cast<float4 *>(smem + kHeadHdrW * kHeadHdrH * 4);           // 68 x 36 threshold texels, fp32 of their fp16 value
@@ -399,27 +392,11 @@ __global__ void __launch_bounds__(kThreads) bloom_head_kernel(const __grid_const
 		{
 			const size_t at = (size_t)y * a.d0.pitch + x;
 			for (int r = 0; r < peers.count; r++)
-				peers.data[r][at] = texel;
+				static_cast<uint2 *>(peers.data[r])[at] = texel;
 		}
 	}
 	if (peers.count != 0)
-	{
-		// publish: every thread's stores are ordered before its CTA's arrival; the last CTA to arrive
-		// raises this rank's flag on every peer
-		__threadfence_system();
-		__syncthreads();
-		if (threadIdx.x == 0)
-		{
-			const unsigned total = gridDim.x * gridDim.y;
-			if (atomicAdd(peers.ctas_done, 1u) == total - 1u)
-			{
-				*peers.ctas_done = 0u;
-				__threadfence_system();
-				for (int r = 0; r < peers.count; r++)
-					asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(peers.flags[r] + peers.flag_index), "r"(peers.epoch) : "memory");
-			}
-		}
-	}
+		peer_publish(peers);
 }
 
 constexpr size_t tent_smem(bool up)
@@ -513,7 +490,7 @@ using namespace grb;
 namespace
 {
 int32_t launch_head(const char *what, const GrbImage *hdr, const float *luminance, const GrbImage *threshold_out, const GrbImage *d0, GrbRows rows,
-                    const HeadPeers &peers, void *stream)
+                    const PeerTargets &peers, void *stream)
 {
 	if (!image_ok(hdr, GRB_FORMAT_B10G11R11_UFLOAT_PACK32, 4) || !d0 || d0->format != GRB_FORMAT_R16G16B16A16_SFLOAT || d0->width <= 0 || d0->height <= 0 ||
 	    (d0->row_pitch % 8) != 0 || (peers.count == 0 && !image_ok(d0, GRB_FORMAT_R16G16B16A16_SFLOAT, 8)) ||
@@ -555,10 +532,7 @@ int32_t launch_head(const char *what, const GrbImage *hdr, const float *luminanc
 	a.inv_t_h = 1.0f / (float)th;
 	a.inv_d0_w = 1.0f / (float)d0->width;
 	a.inv_d0_h = 1.0f / (float)d0->height;
-	// an empty band still has to raise the flags: one CTA with nothing to store (y1 == y0)
-	dim3 grid((d0->width + kOutW - 1) / kOutW, row_count > 0 ? (row_count + kOutH - 1) / kOutH : 1, 1);
-	if (row_count == 0)
-		grid.x = 1;
+	const dim3 grid = peer_grid(row_count, dim3((d0->width + kOutW - 1) / kOutW, (row_count + kOutH - 1) / kOutH, 1));
 	if (luminance)
 		bloom_head_kernel<true><<<grid, kThreads, kHeadSmem, as_stream(stream)>>>(map, a, peers);
 	else
@@ -574,7 +548,7 @@ int32_t launch_head(const char *what, const GrbImage *hdr, const float *luminanc
 extern "C" int32_t grb_bloom_threshold_downsample(const GrbImage *hdr, const float *luminance, const GrbImage *threshold_out, const GrbImage *d0, GrbRows rows,
                                                   void *stream)
 {
-	HeadPeers none{};
+	PeerTargets none{};
 	return launch_head("grb_bloom_threshold_downsample", hdr, luminance, threshold_out, d0, rows, none, stream);
 }
 
@@ -584,25 +558,13 @@ extern "C" int32_t grb_bloom_threshold_downsample_to_peers(const GrbImage *hdr, 
                                                            uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch,
                                                            uint32_t *scratch_counter, GrbRows rows, void *stream)
 {
-	if (!d0_layout || !peer_images || !peer_flags || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS || flag_index < 0)
+	if (!d0_layout)
 	{
-		set_last_error("grb_bloom_threshold_downsample_to_peers: bad arguments");
+		set_last_error("grb_bloom_threshold_downsample_to_peers: null d0_layout");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	HeadPeers peers{};
-	peers.count = peer_count;
-	peers.flag_index = flag_index;
-	peers.epoch = epoch;
-	peers.ctas_done = scratch_counter;
-	for (int r = 0; r < peer_count; r++)
-	{
-		if (!peer_images[r] || !peer_flags[r])
-		{
-			set_last_error("grb_bloom_threshold_downsample_to_peers: null peer pointer");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
-		peers.data[r] = static_cast<uint2 *>(peer_images[r]);
-		peers.flags[r] = peer_flags[r];
-	}
+	PeerTargets peers;
+	if (!peer_targets_from("grb_bloom_threshold_downsample_to_peers", peer_images, peer_flags, peer_count, flag_index, epoch, scratch_counter, peers))
+		return GRB_ERR_INVALID_ARGUMENT;
 	return launch_head("grb_bloom_threshold_downsample_to_peers", hdr, luminance, nullptr, d0_layout, rows, peers, stream);
 }

@@ -510,6 +510,8 @@ dim3 smaa_grid(int w, int rows) { return dim3((unsigned)((w + 31) / 32), (unsign
 } // namespace grb
 
 #ifndef GRB_HOST_EMULATION // tests/cpp/emulate_smaa.cpp compiles the kernels above for the CPU and supplies its own loops
+#include "grb_peer.cuh"
+
 using namespace grb;
 
 extern "C" int32_t grb_smaa_edge_detection(const GrbImage *color, int32_t quality, const GrbImage *edges, GrbRows rows, void *stream)
@@ -530,24 +532,21 @@ extern "C" int32_t grb_smaa_edge_detection(const GrbImage *color, int32_t qualit
 // Row-sharded frames: the weight pass of a rank reads the edges of a window of rows around its band (shard_plan.hpp),
 // most of which other ranks produce.  Each rank computes the edges of its own rows and stores every texel into its
 // own slot image and into the slot image of every peer whose window holds that row (plain 2-byte stores to
-// IPC-mapped peer memory over NVLink), then publishes "rows of frame <epoch> landed" in every rank's flag array --
-// the protocol of bloom_downsample_peers_kernel (grb_post.cu).  The consumer side is grb_peer_wait.
+// IPC-mapped peer memory over NVLink), then publishes "rows of frame <epoch> landed" in every rank's flag array
+// (grb_peer.cuh).  The consumer side is grb_peer_wait.
 namespace grb
 {
 namespace
 {
-struct SmaaEdgeTargets
+// A __grid_constant__ kernel argument: indexed by a run-time rank, it is read from the parameter bank instead of being
+// copied to the stack.
+struct SmaaEdgeWindows
 {
-	uint8_t *data[GRB_MAX_PEERS];
-	uint32_t *flags[GRB_MAX_PEERS];
-	GrbRows window[GRB_MAX_PEERS];
-	int count, self;
+	GrbRows rows[GRB_MAX_PEERS]; // [rank] the edge rows that rank's weight pass reads
 };
 
-__device__ __forceinline__ void smaa_store_release_system(uint32_t *p, uint32_t v) { asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-
-__global__ void __launch_bounds__(256) smaa_edge_peers_kernel(Tex8<4> col, SmaaEdgeTargets t, size_t pitch, SmaaPreset P, int y0, int y1, uint32_t epoch,
-                                                              unsigned *ctas_done)
+__global__ void __launch_bounds__(256) smaa_edge_peers_kernel(Tex8<4> col, PeerTargets t, const __grid_constant__ SmaaEdgeWindows w, size_t pitch,
+                                                              SmaaPreset P, int y0, int y1)
 {
 	const int x = blockIdx.x * 32 + threadIdx.x, y = y0 + blockIdx.y * 8 + threadIdx.y;
 	if (x < col.w && y < y1)
@@ -555,24 +554,10 @@ __global__ void __launch_bounds__(256) smaa_edge_peers_kernel(Tex8<4> col, SmaaE
 		const uchar2 e = smaa_edge_texel(col, P, x, y);
 		const size_t at = (size_t)y * pitch + (size_t)x * 2;
 		for (int q = 0; q < t.count; q++)
-			if (q == t.self || (y >= t.window[q].y0 && y < t.window[q].y1))
-				*reinterpret_cast<uchar2 *>(t.data[q] + at) = e;
+			if (q == t.flag_index || (y >= w.rows[q].y0 && y < w.rows[q].y1))
+				*reinterpret_cast<uchar2 *>(static_cast<uint8_t *>(t.data[q]) + at) = e;
 	}
-	// every thread's stores are ordered before its CTA's arrival; the last CTA to arrive raises this rank's flag on
-	// every rank, also those that take no row from it: each rank waits for all flags (DESIGN.md section 5)
-	__threadfence_system();
-	__syncthreads();
-	if (threadIdx.x == 0 && threadIdx.y == 0)
-	{
-		const unsigned total = gridDim.x * gridDim.y;
-		if (atomicAdd(ctas_done, 1u) == total - 1u)
-		{
-			*ctas_done = 0u;
-			__threadfence_system();
-			for (int q = 0; q < t.count; q++)
-				smaa_store_release_system(t.flags[q] + t.self, epoch);
-		}
-	}
+	peer_publish(t);
 }
 } // namespace
 } // namespace grb
@@ -581,44 +566,35 @@ extern "C" int32_t grb_smaa_edge_detection_to_peers(const GrbImage *color, int32
                                                    uint32_t *const *peer_flags, const GrbRows *peer_windows, int32_t peer_count, int32_t flag_index,
                                                    uint32_t epoch, uint32_t *scratch_counter, GrbRows rows, void *stream)
 {
-	if (!color || !edges_layout || !peer_images || !peer_flags || !peer_windows || !scratch_counter || peer_count < 1 || peer_count > GRB_MAX_PEERS ||
-	    flag_index < 0 || flag_index >= peer_count)
+	if (!color || !edges_layout || !peer_windows)
 	{
-		set_last_error("grb_smaa_edge_detection_to_peers: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1");
+		set_last_error("grb_smaa_edge_detection_to_peers: null pointer");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	PeerTargets t;
+	if (!peer_targets_from("grb_smaa_edge_detection_to_peers", peer_images, peer_flags, peer_count, flag_index, epoch, scratch_counter, t))
+		return GRB_ERR_INVALID_ARGUMENT;
 	if (!rgba8(color) || edges_layout->format != GRB_FORMAT_R8G8_UNORM || edges_layout->width <= 0 || edges_layout->height <= 0 ||
 	    edges_layout->row_pitch < edges_layout->width * 2 || (edges_layout->row_pitch % 2) != 0 || !same_size(color, edges_layout) || quality < 0 || quality > 3)
 	{
 		set_last_error("grb_smaa_edge_detection_to_peers: color R8G8B8A8 (read as UNORM), edges layout R8G8_UNORM of the same size, quality 0..3");
 		return GRB_ERR_UNSUPPORTED_FORMAT;
 	}
-	SmaaEdgeTargets t{};
-	t.count = peer_count;
-	t.self = flag_index;
+	SmaaEdgeWindows windows{};
 	for (int q = 0; q < peer_count; q++)
 	{
 		const GrbRows w = peer_windows[q];
-		if (!peer_images[q] || !peer_flags[q])
-		{
-			set_last_error("grb_smaa_edge_detection_to_peers: null peer pointer");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
 		if (w.y0 < 0 || w.y1 < w.y0 || w.y1 > edges_layout->height)
 		{
 			set_last_error("grb_smaa_edge_detection_to_peers: a peer's edge window lies outside the image (0 <= y0 <= y1 <= height)");
 			return GRB_ERR_INVALID_ARGUMENT;
 		}
-		t.data[q] = static_cast<uint8_t *>(peer_images[q]);
-		t.flags[q] = peer_flags[q];
-		t.window[q] = w;
+		windows.rows[q] = w;
 	}
 	rows = full_rows(rows, edges_layout->height);
-	// an empty band still has to raise the flags: one CTA with nothing to store
 	const int row_count = rows.y1 > rows.y0 ? rows.y1 - rows.y0 : 0;
-	const dim3 grid = row_count > 0 ? smaa_grid(edges_layout->width, row_count) : dim3(1, 1, 1);
-	smaa_edge_peers_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(tex_of<4>(color), t, (size_t)edges_layout->row_pitch, preset_of(quality), rows.y0,
-	                                                                    rows.y0 + row_count, epoch, scratch_counter);
+	smaa_edge_peers_kernel<<<peer_grid(row_count, smaa_grid(edges_layout->width, row_count)), dim3(32, 8), 0, as_stream(stream)>>>(
+	    tex_of<4>(color), t, windows, (size_t)edges_layout->row_pitch, preset_of(quality), rows.y0, rows.y0 + row_count);
 	return check_launch("grb_smaa_edge_detection_to_peers");
 }
 

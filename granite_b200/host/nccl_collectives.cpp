@@ -86,10 +86,8 @@ bool nccl_ok(int rc, const char *what)
 
 NcclCollectives::~NcclCollectives()
 {
-	release_peer_exchange(bloom_d0);
-	release_peer_exchange(smaa_edge);
-	release_peer_exchange(taa_history);
-	release_peer_exchange(present);
+	for (PeerState &channel : channels)
+		release_peer_exchange(channel);
 	if (comm && api().CommDestroy)
 		api().CommDestroy(comm);
 }
@@ -274,28 +272,9 @@ bool NcclCollectives::setup_peer_exchange(PeerState &peer, size_t image_bytes)
 	return true;
 }
 
-bool NcclCollectives::peer_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+bool NcclCollectives::peer_exchange_begin_frame(PeerChannel channel, size_t image_bytes, PeerSlot &slot)
 {
-	return begin_frame(bloom_d0, image_bytes, slot);
-}
-
-bool NcclCollectives::smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-{
-	return begin_frame(smaa_edge, image_bytes, slot);
-}
-
-bool NcclCollectives::taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-{
-	return begin_frame(taa_history, image_bytes, slot);
-}
-
-bool NcclCollectives::present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-{
-	return begin_frame(present, image_bytes, slot);
-}
-
-bool NcclCollectives::begin_frame(PeerState &peer, size_t image_bytes, PeerSlot &slot)
-{
+	PeerState &peer = channels[(size_t)channel];
 	if (!peer.tried || (peer.ok && peer.image_bytes != image_bytes))
 	{
 		// (a re-bake at another size re-creates the buffers; all ranks re-bake together)

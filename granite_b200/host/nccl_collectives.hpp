@@ -27,13 +27,7 @@ public:
 	bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) override;
 	// Peer-memory exchange: two image slots + a flag array per rank, cudaIpc-mapped into every
 	// other rank (handles are exchanged with one ncclAllGather).  GRB_SHARD_EXCHANGE=nccl disables it.
-	bool peer_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
-	// Second channel, same set-up and teardown: the SMAA edge rows (host/post/smaa.cpp).
-	bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
-	// Third channel: the TAA history (host/post/temporal.cpp).
-	bool taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
-	// Fourth channel: the bands of the final image, pushed to the presenting rank (host/scene_viewer.cpp).
-	bool present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot) override;
+	bool peer_exchange_begin_frame(PeerChannel channel, size_t image_bytes, PeerSlot &slot) override;
 
 private:
 	bool collective_failed(const char *what);
@@ -51,11 +45,7 @@ private:
 		std::vector<void *> opened;
 		uint32_t epoch = 0;
 	};
-	PeerState bloom_d0;  // bloom d0 bands
-	PeerState smaa_edge; // SMAA edge rows
-	PeerState taa_history; // TAA history rows
-	PeerState present;     // the final image on the presenting rank
-	bool begin_frame(PeerState &channel, size_t image_bytes, PeerSlot &slot);
+	PeerState channels[(size_t)PeerChannel::Present + 1]; // [PeerChannel]
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);
 };

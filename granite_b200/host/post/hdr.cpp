@@ -58,7 +58,8 @@ void bloom_build_compute(Vulkan::CommandBuffer &cmd, RenderGraph &graph, const F
 	// broadcasts after a local pass.  The unfused pair remains for shapes the tile kernel does not cover.
 	const bool keep_threshold = getenv("GRB_BLOOM_KEEP_THRESHOLD") != nullptr;
 	RenderGraphCollectives::PeerSlot slot;
-	const bool peer_stores = sharded && graph.get_collectives()->peer_exchange_begin_frame((size_t)d0.row_pitch * (size_t)d0.height, slot);
+	const bool peer_stores = sharded && graph.get_collectives()->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::BloomD0,
+	                                                                                       (size_t)d0.row_pitch * (size_t)d0.height, slot);
 	if (peer_stores)
 	{
 		const unsigned self = graph.get_collectives()->get_rank();
@@ -84,12 +85,7 @@ void bloom_build_compute(Vulkan::CommandBuffer &cmd, RenderGraph &graph, const F
 	graph.signal_mark("bloom-head", cmd);
 
 	if (sharded && !peer_stores)
-	{
-		std::vector<GrbRows> bands;
-		for (unsigned rank = 0; rank < graph.get_shard_count(); rank++)
-			bands.push_back(graph.get_shard_plan(rank).downsample0);
-		graph.get_collectives()->all_gather_rows(cmd, graph.get_physical_texture_resource(*r.d0), bands);
-	}
+		graph.get_collectives()->all_gather_rows(cmd, graph.get_physical_texture_resource(*r.d0), graph.get_shard_plan_rows(&ShardPlan::downsample0));
 
 	// d3 blends with its own previous frame (hdr.cpp:156-167, 182): lerp = 1 - 0.001^frame_time;
 	// luminance_build_compute (hdr.cpp:68-98): size = d3 / 2, lerp = 1 - 0.5^frame_time, clamp [-3, 2]

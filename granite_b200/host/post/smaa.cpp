@@ -200,25 +200,19 @@ void setup_smaa_postprocess(RenderGraph &graph, TemporalJitter &jitter, float, c
 		GrbImage edges = edge_view.as_grb();
 		void *stream = cmd.get_stream_handle();
 		const bool sharded = graph.is_sharded() && graph.get_shard_count() > 1;
-		exchange->peer_stores = sharded &&
-		                        graph.get_collectives()->smaa_edge_exchange_begin_frame((size_t)edges.row_pitch * (size_t)edges.height, exchange->slot);
+		exchange->peer_stores = sharded && graph.get_collectives()->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::SmaaEdges,
+		                                                                                      (size_t)edges.row_pitch * (size_t)edges.height, exchange->slot);
 		if (!sharded)
 		{
 			cmd.check(grb_smaa_edge_detection(&color, quality, &edges, GrbRows{ 0, 0 }, stream), "grb_smaa_edge_detection");
 			return;
 		}
-		const unsigned ranks = graph.get_shard_count();
-		std::vector<GrbRows> windows, bands;
-		for (unsigned r = 0; r < ranks; r++)
-		{
-			const ShardPlan p = graph.get_shard_plan(r);
-			windows.push_back(p.smaa_edge_window);
-			bands.push_back(p.smaa_edges);
-		}
+		const std::vector<GrbRows> bands = graph.get_shard_plan_rows(&ShardPlan::smaa_edges);
 		const unsigned self = graph.get_shard_rank();
 		if (exchange->peer_stores)
 		{
 			const auto &slot = exchange->slot;
+			const std::vector<GrbRows> windows = graph.get_shard_plan_rows(&ShardPlan::smaa_edge_window);
 			cmd.check(grb_smaa_edge_detection_to_peers(&color, quality, &edges, slot.images, slot.flags, windows.data(), (int32_t)slot.count, (int32_t)self,
 			                                           slot.epoch, slot.counter, bands[self], stream),
 			          "grb_smaa_edge_detection_to_peers");

@@ -153,8 +153,8 @@ void setup_taa_resolve(RenderGraph &graph, TemporalJitter &jitter, float scaling
 		const ShardPlan plan = graph.get_shard_plan();
 		const RenderGraphCollectives::PeerSlot last = exchange->slot;
 		const bool had_slot = exchange->peer_stores;
-		exchange->peer_stores =
-		    graph.get_collectives()->taa_history_exchange_begin_frame((size_t)oh.row_pitch * (size_t)oh.height, exchange->slot);
+		exchange->peer_stores = graph.get_collectives()->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::TaaHistory,
+		                                                                           (size_t)oh.row_pitch * (size_t)oh.height, exchange->slot);
 		if (exchange->peer_stores)
 		{
 			// Every rank stores its own history rows into every rank's slot of this frame, and reads last frame's slot
@@ -175,10 +175,7 @@ void setup_taa_resolve(RenderGraph &graph, TemporalJitter &jitter, float scaling
 		// without peer memory: the TAA rows here (the exact kernel: explicit rows), then every rank's produced history
 		// rows (its own band, or its render rows under FSR) to every rank
 		cmd.check(grb_taa_resolve(&image, &depth, &image_mv, prev ? &prev_img : nullptr, reproj.data(), q, &oc, &oh, plan.taa, stream), "grb_taa_resolve");
-		std::vector<GrbRows> bands;
-		for (unsigned r = 0; r < graph.get_shard_count(); r++)
-			bands.push_back(graph.get_shard_plan(r).render_own);
-		graph.get_collectives()->all_gather_rows(cmd, history_view, bands);
+		graph.get_collectives()->all_gather_rows(cmd, history_view, graph.get_shard_plan_rows(&ShardPlan::render_own));
 	});
 }
 } // namespace Granite

@@ -56,6 +56,16 @@ public:
 	// this frame's slot: the copy's address on every rank as seen from this device, every rank's
 	// flag array, and the epoch to publish / wait for.  false = not available (single process
 	// without peer access, IPC refused...): callers then use all_gather_rows().
+	// Each channel is independent: its own two slots, flag arrays, counter and epoch.
+	enum class PeerChannel
+	{
+		BloomD0,    // the bloom d0 bands (host/post/hdr.cpp)
+		SmaaEdges,  // the SMAA edge rows each rank's weight pass reads around its band (host/post/smaa.cpp)
+		TaaHistory, // the whole TAA history, each rank producing its own rows; the next frame reads the slot this frame
+		            // filled (host/post/temporal.cpp)
+		Present,    // the bands of the final image, pushed into the presenting rank's slots only (the "present" pass of
+		            // scene_viewer.cpp)
+	};
 	struct PeerSlot
 	{
 		void *images[8] = {};     // [rank] base address of this frame's slot on that rank
@@ -64,32 +74,9 @@ public:
 		uint32_t epoch = 0;
 		unsigned count = 0;
 	};
-	virtual bool peer_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
+	virtual bool peer_exchange_begin_frame(PeerChannel channel, size_t image_bytes, PeerSlot &slot)
 	{
-		(void)image_bytes;
-		(void)slot;
-		return false;
-	}
-	// The same exchange on a second, independent channel (its own two slots, flag arrays, counter and epoch) for the
-	// SMAA edge rows, which a frame exchanges besides the bloom d0 bands (host/post/smaa.cpp).
-	virtual bool smaa_edge_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-	{
-		(void)image_bytes;
-		(void)slot;
-		return false;
-	}
-	// A third channel for the TAA history (host/post/temporal.cpp): every rank's slot holds the whole history image,
-	// each rank produces its own rows of it, and the next frame reads the slot this frame filled.
-	virtual bool taa_history_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-	{
-		(void)image_bytes;
-		(void)slot;
-		return false;
-	}
-	// A fourth channel for presenting a sharded frame from one rank (the "present" pass of scene_viewer.cpp): only the
-	// presenting rank's slots are written, each rank pushing its band of the final image into them.
-	virtual bool present_exchange_begin_frame(size_t image_bytes, PeerSlot &slot)
-	{
+		(void)channel;
 		(void)image_bytes;
 		(void)slot;
 		return false;
@@ -499,6 +486,14 @@ public:
 	{
 		return compute_shard_plan(swapchain_dimensions.width, swapchain_dimensions.height, shard_bands, rank, shard_fxaa, shard_smaa_quality, shard_taa,
 		                          shard_upscale);
+	}
+	// One field of every rank's plan, indexed by rank (e.g. the rows each rank produces, for all_gather_rows).
+	std::vector<GrbRows> get_shard_plan_rows(GrbRows ShardPlan::*field) const
+	{
+		std::vector<GrbRows> rows;
+		for (unsigned r = 0; r < get_shard_count(); r++)
+			rows.push_back(get_shard_plan(r).*field);
+		return rows;
 	}
 	GrbRows shard_rows_for(unsigned resource_height, unsigned halo_rows = 0) const;
 	GrbRows shard_rows_for_rank(unsigned rank, unsigned resource_height, unsigned halo_rows = 0) const;

@@ -386,7 +386,8 @@ void GrbhViewer::bake_render_graph()
 			void *stream = cmd.get_stream_handle();
 			const unsigned P = (unsigned)present_rank;
 			RenderGraphCollectives::PeerSlot slot;
-			if (graph.get_collectives()->present_exchange_begin_frame((size_t)image.row_pitch * (size_t)image.height, slot))
+			if (graph.get_collectives()->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::Present, (size_t)image.row_pitch * (size_t)image.height,
+			                                                       slot))
 			{
 				// the credit: P's push of the last frame ran after P's readback of the frame before, the last one that
 				// used this frame's slot

@@ -297,13 +297,16 @@ int32_t grb_bloom_threshold_downsample(const GrbImage *hdr, const float *luminan
  * peer memory over NVLink / NVSwitch; one entry is this rank's own image), all with out_layout's
  * size and pitch -- and then flags[flag_index] = epoch is release-stored into every rank's flag
  * array.  scratch_counter: one zero-initialised uint32 in local device memory.  No reference
- * equivalent (the reference never splits a frame). */
+ * equivalent (the reference never splits a frame).
+ * GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside
+ * 0..peer_count-1 (checked before any CUDA call; nothing is written). */
 #define GRB_MAX_PEERS 8
 int32_t grb_bloom_downsample_to_peers(const GrbImage *in, const GrbImage *out_layout, void *const *peer_images,
                                       uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch,
                                       uint32_t *scratch_counter, GrbRows rows, void *stream);
 /* grb_bloom_threshold_downsample with the same exchange fused in (threshold tile in shared memory, d0
- * band stored to every rank, flags raised).  Same eligibility rule; GRB_ERR_UNSUPPORTED_FORMAT otherwise. */
+ * band stored to every rank, flags raised).  Same eligibility rule; GRB_ERR_UNSUPPORTED_FORMAT otherwise.
+ * GRB_ERR_INVALID_ARGUMENT as grb_bloom_downsample_to_peers. */
 int32_t grb_bloom_threshold_downsample_to_peers(const GrbImage *hdr, const float *luminance, const GrbImage *d0_layout,
                                                 void *const *peer_images, uint32_t *const *peer_flags, int32_t peer_count,
                                                 int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, GrbRows rows,

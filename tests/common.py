@@ -6,6 +6,16 @@ import numpy as np
 from granite_b200 import synth
 
 
+def free_port() -> int:
+    """A TCP port nothing listens on now, for the rendezvous of a torchrun launch.  A fixed port fails with EADDRINUSE
+    whenever another run on the same host holds it."""
+    import socket
+
+    with socket.socket() as s:
+        s.bind(("", 0))
+        return s.getsockname()[1]
+
+
 def build_case(oracle, width, height, n_lights, spot_fraction=0.0):
     """Scene + oracle host prep (camera, light records, cluster params) for one config."""
     scene = synth.make_scene(width, height)

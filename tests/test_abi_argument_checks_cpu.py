@@ -141,3 +141,37 @@ def test_fog_light_density_argument_checks(lib):
     assert lib.grb_fog_light_density(*args(bad, p(buf))) == ERR_ARG
     bad = capi.GrbFogParameters(8, 4, 4, 0, 0.0, 0.5, 1.0)
     assert lib.grb_fog_light_density(*args(bad, p(buf))) == ERR_ARG
+
+
+def test_bloom_to_peers_argument_checks(lib):
+    """Both bloom d0 exchanges refuse a flag_index outside 0..peer_count-1 (word peer_count onwards of a flag array may
+    hold the scratch counter), a null peer pointer and a peer_count outside 1..GRB_MAX_PEERS, and write nothing."""
+    from granite_b200 import capi
+
+    keep = [np.zeros((16, 32), np.uint32), np.zeros((8, 16, 4), np.uint16)] + [np.zeros((4, 8, 4), np.uint16) for _ in range(8)] + \
+           [np.zeros(16, np.uint32) for _ in range(8)]
+    hdr = _image(capi, keep[0], capi.FORMAT_B10G11R11_UFLOAT)
+    t = _image(capi, keep[1], capi.FORMAT_R16G16B16A16_SFLOAT)
+    d0 = capi.GrbImage(None, 8, 4, 8 * 8, capi.FORMAT_R16G16B16A16_SFLOAT)
+    images = (C.c_void_p * 8)(*[a.ctypes.data for a in keep[2:10]])
+    flags = (C.c_void_p * 8)(*[a.ctypes.data for a in keep[10:]])
+    counter = C.c_void_p(keep[10].ctypes.data + 32)
+
+    def head(im=images, fl=flags, n=2, k=0):
+        return lib.grb_bloom_threshold_downsample_to_peers(C.byref(hdr), None, C.byref(d0), im, fl, n, k, C.c_uint32(1), counter, capi.GrbRows(0, 4), None)
+
+    def down(im=images, fl=flags, n=2, k=0):
+        return lib.grb_bloom_downsample_to_peers(C.byref(t), C.byref(d0), im, fl, n, k, C.c_uint32(1), counter, capi.GrbRows(0, 4), None)
+
+    null_image = (C.c_void_p * 8)(keep[2].ctypes.data, None)
+    null_flags = (C.c_void_p * 8)(None, keep[11].ctypes.data)
+    for call, name in ((head, "grb_bloom_threshold_downsample_to_peers"), (down, "grb_bloom_downsample_to_peers")):
+        assert call(k=2) == ERR_ARG and name in _msg(lib) and "flag_index" in _msg(lib)
+        assert call(n=8, k=8) == ERR_ARG
+        assert call(k=-1) == ERR_ARG
+        assert call(im=null_image) == ERR_ARG and "null peer" in _msg(lib)
+        assert call(fl=null_flags) == ERR_ARG and "null peer" in _msg(lib)
+        assert call(im=None) == ERR_ARG
+        assert call(n=0) == ERR_ARG and "peer_count" in _msg(lib)
+        assert call(n=9) == ERR_ARG and "peer_count" in _msg(lib)
+    assert all(a.sum() == 0 for a in keep[2:])

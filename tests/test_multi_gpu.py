@@ -10,6 +10,8 @@ import sys
 
 import pytest
 
+from tests import common
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -25,7 +27,7 @@ def _gpu_count():
 def test_sharded_frame_is_bit_identical(cuda, fxaa, exchange):
     world = 4 if _gpu_count() >= 4 else 2
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(29511 + fxaa + (2 if exchange == "nccl" else 0)), os.path.join(ROOT, "tests", "multi_gpu_worker.py"), "1280", "768", "300", str(fxaa)]
+           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_worker.py"), "1280", "768", "300", str(fxaa)]
     env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
     proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
     try:

@@ -5,7 +5,6 @@ through its C entry point), the all-gather of 1/4-res bloom bands and the zero-p
 that assembles the luminance grid exactly.  A plan with a halo one row too small would leak
 never-computed (zero) rows into a band and break the bit-equality asserted here."""
 import os
-import socket
 
 import numpy as np
 import pytest
@@ -13,15 +12,9 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from tests import common
+
 W, H, N_LIGHTS = 512, 384, 64  # 6 bands of 64 rows
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _reference_frame(oracle, scene, cam, prep):
@@ -111,7 +104,7 @@ def test_two_rank_gloo_frame_equals_single_rank(oracle, fxaa):
     expect = ldr_fxaa if fxaa else f.ldr
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = common.free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, fxaa, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -9,6 +9,8 @@ import sys
 import numpy as np
 import pytest
 
+from tests import common
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SENTINEL = 0x3C3C3C3C
@@ -72,7 +74,7 @@ def test_presented_sharded_frame_is_bit_identical(cuda, exchange):
     unsharded frame, and the other ranks return their bands."""
     from tests.multi_gpu_present_worker import CONFIGS, FRAMES, RUNS
 
-    rc, out, err = _run_worker(exchange, 29561 + (1 if exchange == "nccl" else 0))
+    rc, out, err = _run_worker(exchange, common.free_port())
     assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count("tonemap-only sharded == single GPU: True") == 2 * FRAMES, out[-3000:]
     assert out.count("presented == single GPU: True") == len(CONFIGS) * len(RUNS) * FRAMES, out[-3000:]

@@ -79,7 +79,7 @@ def test_sharded_taa_frame_is_bit_identical(cuda, exchange):
     narrow bands; 6 frames each with a moving camera and large vertical motion vectors."""
     world = 4
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(29541 + (1 if exchange == "nccl" else 0)), os.path.join(ROOT, "tests", "multi_gpu_taa_worker.py"), "1280", "768", "300"]
+           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_taa_worker.py"), "1280", "768", "300"]
     env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
     proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
     try:

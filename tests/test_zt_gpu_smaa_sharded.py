@@ -9,6 +9,7 @@ import sys
 import numpy as np
 import pytest
 
+from tests import common
 from tests.test_oracle_ref_smaa import smaa_test_image
 
 pytestmark = pytest.mark.gpu
@@ -71,7 +72,7 @@ def test_sharded_smaa_frame_is_bit_identical(cuda, exchange):
     """4 ranks (sharing GPUs where there are fewer), equal and narrow bands, presets Low and Ultra, 4 frames each."""
     world = 4
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(29531 + (1 if exchange == "nccl" else 0)), os.path.join(ROOT, "tests", "multi_gpu_smaa_worker.py"), "1280", "768", "300"]
+           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_smaa_worker.py"), "1280", "768", "300"]
     env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
     proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
     try:
