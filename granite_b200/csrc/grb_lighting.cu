@@ -398,17 +398,18 @@ struct Surface2
 	f2 m2m1, cgd, omk, k, Vk, NoVr;
 };
 
-// dk + F * (G*D - dk) per channel for both pixels; NoL returned for the caller's weight.
-__device__ __forceinline__ void brdf2(const Surface2 &s, f2 NoLr, f2 VoL, f2 &NoL, f2 &tx, f2 &ty, f2 &tz)
+// dk + F * (G*D - dk) per channel for both pixels and the (unnormalised) half vector h = V + L; NoL returned for
+// the caller's weight.  h is formed explicitly, as in brdf(): from |V+L|^2 = 2 + 2 V.L the grazing specular peak
+// (L near -V) loses all precision.
+__device__ __forceinline__ void brdf2(const Surface2 &s, f2 hx, f2 hy, f2 hz, f2 &NoL, f2 &tx, f2 &ty, f2 &tz)
 {
-	// NoLr = N.L and VoL = V.L for unit L; the half vector is never formed:
-	// |V+L|^2 = 2 + 2 VoL,  N.(V+L) = NoV + NoL,  V.(V+L) = 1 + VoL
-	f2 inv_h = rsqrt2(fma2(VoL, mk2(2.0f), mk2(2.0f)));
-	NoL = clamp2(NoLr, 0.001f, 1.0f);
-	f2 NoH = clamp2(mul2(add2(NoLr, s.NoVr), inv_h), 0.0001f, 1.0f);
-	f2 HoV = fma2(VoL, inv_h, inv_h); // <= 1 up to rounding, see brdf()
-	HoV = make_float2(fmaxf(HoV.x, 0.001f), fmaxf(HoV.y, 0.001f));
-	f2 f = fma2(HoV, mk2(-1.0f), mk2(1.0f));
+	f2 hh = dot3_2(hx, hy, hz, hx, hy, hz);
+	f2 inv_h = rsqrt2(hh);
+	f2 Nh = dot3_2(s.Nx, s.Ny, s.Nz, hx, hy, hz);
+	NoL = clamp2(add2(Nh, make_float2(-s.NoVr.x, -s.NoVr.y)), 0.001f, 1.0f); // N.L = N.h - N.V
+	f2 NoH = clamp2(mul2(Nh, inv_h), 0.0001f, 1.0f);
+	f2 f = fma2(mul2(hh, inv_h), mk2(-0.5f), mk2(1.0f)); // 1 - max(HoV, 0.001), HoV = |h| / 2
+	f = make_float2(fminf(f.x, 0.999f), fminf(f.y, 0.999f));
 	f2 fsq = mul2(f, f);
 	f2 f5 = mul2(mul2(fsq, fsq), f);
 	f2 d = fma2(mul2(NoH, NoH), s.m2m1, mk2(1.0f));
@@ -570,7 +571,6 @@ __device__ __forceinline__ void walk_lights(const LightingParams &p, const PairS
 			f2 t = fma2(xr, mk2(1.0f / (1.0f - 0.9f)), mk2(-0.9f / (1.0f - 0.9f)));
 			t = make_float2(__saturatef(t.x), __saturatef(t.y));
 			f2 falloff = fma2(mul2(mul2(t, t), fma2(mk2(-2.0f), t, mk2(3.0f))), mk2(-1.0f), mk2(1.0f));
-			// L = l * inv_d is never formed either: every use of it is a dot product
 			if (!((tm >> bit) & 1u))
 			{
 				float2 sb = __half22float2(*reinterpret_cast<const __half2 *>(&l0.w));
@@ -579,10 +579,8 @@ __device__ __forceinline__ void walk_lights(const LightingParams &p, const PairS
 				cone = make_float2(__saturatef(cone.x), __saturatef(cone.y));
 				falloff = mul2(falloff, mul2(cone, cone));
 			}
-			f2 NoLr = mul2(dot3_2(s.Nx, s.Ny, s.Nz, lx, ly, lz), inv_d);
-			f2 VoL = mul2(dot3_2(s.Vx, s.Vy, s.Vz, lx, ly, lz), inv_d);
 			f2 NoL, tx, ty, tz;
-			brdf2(s, NoLr, VoL, NoL, tx, ty, tz);
+			brdf2(s, fma2(lx, inv_d, s.Vx), fma2(ly, inv_d, s.Vy), fma2(lz, inv_d, s.Vz), NoL, tx, ty, tz);
 			f2 w = mul2(mul2(NoL, falloff), mul2(inv_ld, inv_ld));
 			// a lane outside the light's mask or radius adds exactly 0 (falloff is 0 beyond the radius)
 			w = make_float2(nearA ? w.x : 0.0f, nearB ? w.y : 0.0f);
@@ -616,7 +614,7 @@ __global__ void __launch_bounds__(32 * kWarpsPerCta, 5) deferred_lighting2_kerne
 		const Surface2 &s = q.s;
 		f2 NoL, tx, ty, tz;
 		const f2 dx = mk2(p.dir_dir.x), dy = mk2(p.dir_dir.y), dz = mk2(p.dir_dir.z);
-		brdf2(s, dot3_2(s.Nx, s.Ny, s.Nz, dx, dy, dz), dot3_2(s.Vx, s.Vy, s.Vz, dx, dy, dz), NoL, tx, ty, tz);
+		brdf2(s, add2(s.Vx, dx), add2(s.Vy, dy), add2(s.Vz, dz), NoL, tx, ty, tz);
 		if (A.lit)
 		{
 			float3 e = unpack_r11g11b10(dstA);
@@ -720,7 +718,6 @@ struct PersistentArgs
 	uint32_t *schedule; // optional: [blocks_x, blocks_y, valid, 0][max block cost per strip][strips by falling cost][block shape per strip]
 	unsigned rec_bytes; // n_lights * 48, multiple of 16
 	unsigned row_shape_threshold; // 0 = every strip uses 16x4 blocks (default); else cost (cycles >> 5) above which a strip switches to 64x1 blocks
-	int use_bulk_copy;
 };
 
 struct SurfaceP
@@ -822,29 +819,20 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 			s_order[i] = (uint16_t)(strip | (a.schedule[4 + 2 * a.blocks_y + strip] ? 0x8000u : 0u));
 		}
 	__syncthreads();
-	if (a.use_bulk_copy)
+	// the light table (16-byte aligned, launch_deferred_lighting checks it) by the bulk-copy engine
+	if (threadIdx.x == 0 && a.rec_bytes)
 	{
-		if (threadIdx.x == 0 && a.rec_bytes)
+		asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(a.rec_bytes) : "memory");
+		const unsigned char *src = reinterpret_cast<const unsigned char *>(p.lights);
+		for (unsigned off = 0; off < a.rec_bytes; off += 32768u)
 		{
-			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(a.rec_bytes) : "memory");
-			const unsigned char *src = reinterpret_cast<const unsigned char *>(p.lights);
-			for (unsigned off = 0; off < a.rec_bytes; off += 32768u)
-			{
-				const unsigned n = min(32768u, a.rec_bytes - off);
-				asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_raw + off)),
-				             "l"(src + off), "r"(n), "r"(bar)
-				             : "memory");
-			}
+			const unsigned n = min(32768u, a.rec_bytes - off);
+			asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(smem_raw + off)),
+			             "l"(src + off), "r"(n), "r"(bar)
+			             : "memory");
 		}
 	}
-	else
-	{
-		const float4 *src = reinterpret_cast<const float4 *>(p.lights);
-		for (unsigned i = threadIdx.x; i < a.rec_bytes / 16u; i += blockDim.x)
-			s_rec[i] = __ldg(src + i);
-		__syncthreads();
-	}
-	bool table_ready = !a.use_bulk_copy || a.rec_bytes == 0;
+	bool table_ready = a.rec_bytes == 0;
 
 	uint16_t *list = s_lists + warp * (kListCap + 2);
 	const unsigned dummy_entry = (unsigned)a.n_lights;
@@ -1496,6 +1484,12 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		set_last_error("grb_deferred_lighting: null cluster_range");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	if (reinterpret_cast<uintptr_t>(buf->lights) % 16 != 0)
+	{
+		// every form reads the records as float4 (and the persistent one bulk-copies them)
+		set_last_error("grb_deferred_lighting: lights must be 16-byte aligned");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
 	rows = full_rows(rows, h);
 	if (rows.y1 <= rows.y0)
 		return GRB_OK;
@@ -1598,7 +1592,6 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		a.schedule = static_cast<uint32_t *>(schedule);
 		a.n_lights = params->num_lights;
 		a.rec_bytes = (unsigned)params->num_lights * 48u;
-		a.use_bulk_copy = (reinterpret_cast<uintptr_t>(buf->lights) % 16) == 0 ? 1 : 0;
 		{
 			// experiment, off by default: measured on the bench scene the one-row blocks execute 7 % MORE instructions (their
 			// lists are not shorter: depth varies along x as much as across 4 rows there) -- DESIGN.md section 4
@@ -1675,6 +1668,11 @@ extern "C" int32_t grb_lighting_row_cost(const GrbImage *depth, const GrbCamera 
 	if (!buf->cluster_range || (params->num_lights > 0 && (!buf->lights || !buf->bitmask)))
 	{
 		set_last_error("grb_lighting_row_cost: null cluster buffer");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (reinterpret_cast<uintptr_t>(buf->lights) % 16 != 0)
+	{
+		set_last_error("grb_lighting_row_cost: lights must be 16-byte aligned");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	rows = full_rows(rows, depth->height);

@@ -135,6 +135,13 @@ def deferred_lighting(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDe
                                                 C.byref(img), capi.rows(rows), capi.stream_ptr()), "grb_deferred_lighting")
 
 
+def deferred_lighting_blocks(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDevice, hdr: torch.Tensor, rows=None):
+    """grb_deferred_lighting_blocks: the pass as a grid of short-lived CTAs (the form row-sharded frames may use)."""
+    img = _hdr_img(hdr)
+    capi.check(capi.lib().grb_deferred_lighting_blocks(C.byref(gb.struct), C.byref(cam), C.byref(cluster.params), C.byref(cluster.buffers),
+                                                       C.byref(img), capi.rows(rows), capi.stream_ptr()), "grb_deferred_lighting_blocks")
+
+
 def deferred_lighting_shadowed(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDevice, transforms: torch.Tensor, map_table: torch.Tensor,
                               resolution: int, hdr: torch.Tensor, rows=None, pcf_wide=False):
     """Lighting with shadowed positional lights.  transforms: float32 (n, 16) device tensor (cluster order); map_table: int64 (n,)

@@ -121,7 +121,7 @@ typedef struct GrbCamera
  * path reads (math/render_parameters.hpp:155-162), passed as separate device arrays. */
 typedef struct GrbClusterBuffers
 {
-	const GrbPositionalLight *lights; /* num_lights */
+	const GrbPositionalLight *lights; /* num_lights, 16-byte aligned (the lighting pass reads records as float4) */
 	const float *model;               /* num_lights x 12: mat_affine rows */
 	const uint32_t *type_mask;        /* num_lights_32 words, bit = 1 => point light */
 	const uint32_t *z_ranges;         /* max(num_lights,1) x uvec2, host-computed (clusterer.cpp:1322-1346) */

@@ -11,6 +11,8 @@ Cases:
   chain       the viewer's post chain on a fixed HDR image (the oracle's lit frame as emissive, no lights, sky
               everywhere) at 640x360 and 3840x2160, 3 frames: the frame, every pyramid level and average-luminance
   zrange      grb_cluster_build for 300 lights (25 % spots) at the 640x360 aspect: cluster-bitmask and cluster-range
+  lighting    grb_deferred_lighting on the 640x360 / 300 lights / 25 % spots case, then three grb_deferred_lighting_scheduled
+              launches on one schedule buffer: each frame, and the schedule after each launch
 """
 import os
 import sys
@@ -22,7 +24,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-SWITCHES = ("GRB_POST_EXACT", "GRB_POST_NO_TILES", "GRB_BLOOM_NO_FUSED_TAIL", "GRB_BLOOM_TAIL_CTAS", "GRB_ZRANGE_SCAN")
+SWITCHES = ("GRB_POST_EXACT", "GRB_POST_NO_TILES", "GRB_BLOOM_NO_FUSED_TAIL", "GRB_BLOOM_TAIL_CTAS", "GRB_ZRANGE_SCAN", "GRB_LIGHTING_V2",
+            "GRB_LIGHTING_1PX", "GRB_LIGHTING_ROW_BLOCKS")
+LIGHTING_CASE = (640, 360, 300, 0.25)
 CHAIN_SIZES = ((640, 360), (3840, 2160))
 CHAIN_FRAMES = 3
 PYRAMID = ("downsample-0", "downsample-1", "downsample-2", "downsample-3", "upsample-2", "upsample-1", "upsample-0")
@@ -120,6 +124,37 @@ def zrange(out_dir):
     np.savez(os.path.join(out_dir, "zrange.npz"), bitmask=got.bitmask, range=got.range)
 
 
+def lighting_device_case(oracle):
+    """Scene, device G-buffer, device cluster (built by grb_cluster_build) and camera of LIGHTING_CASE."""
+    from granite_b200 import harness
+    from tests import common
+
+    scene, cam, _, prep = common.build_case(oracle, *LIGHTING_CASE)
+    dev = harness.ClusterDevice(prep.records, prep.model, prep.type_mask, prep.z_ranges, prep.params, prep.res)
+    gcam = harness.camera_struct(cam)
+    dev.build(gcam)
+    return scene, harness.GBufferDevice(scene), dev, gcam
+
+
+def lighting(out_dir):
+    from granite_b200 import harness
+    from oracle import pyoracle as oracle
+
+    oracle.build(ref=False)
+    scene, gb, dev, gcam = lighting_device_case(oracle)
+    res = {}
+    hdr = gb.emissive.clone()
+    harness.deferred_lighting(gb, gcam, dev, hdr)
+    res["default"] = harness.to_host(hdr, np.uint32)
+    sched = harness.lighting_schedule(scene.depth.shape[0])
+    for i in range(3):
+        hdr = gb.emissive.clone()
+        harness.deferred_lighting(gb, gcam, dev, hdr, schedule=sched)
+        res[f"{i}/scheduled"] = harness.to_host(hdr, np.uint32)
+        res[f"{i}/schedule"] = harness.to_host(sched, np.uint32)
+    np.savez(os.path.join(out_dir, "lighting.npz"), **res)
+
+
 def main():
     case, out_dir = sys.argv[1], sys.argv[2]
     seen = " ".join(f"{k}={os.environ[k]}" for k in SWITCHES if k in os.environ)
@@ -129,7 +164,7 @@ def main():
 
     capi.lib()
     capi.init()
-    {"post_exact": post_exact, "chain": chain, "zrange": zrange}[case](out_dir)
+    {"post_exact": post_exact, "chain": chain, "zrange": zrange, "lighting": lighting}[case](out_dir)
     torch.cuda.synchronize()
     print(f"{case}: done", flush=True)
 

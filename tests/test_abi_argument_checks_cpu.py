@@ -175,3 +175,35 @@ def test_bloom_to_peers_argument_checks(lib):
         assert call(n=0) == ERR_ARG and "peer_count" in _msg(lib)
         assert call(n=9) == ERR_ARG and "peer_count" in _msg(lib)
     assert all(a.sum() == 0 for a in keep[2:])
+
+
+def test_lighting_rejects_misaligned_lights(lib):
+    """Every lighting form reads the light records as float4, so a light table that is not 16-byte aligned is refused
+    before any CUDA call, by the lighting pass and by its row-cost estimate."""
+    from granite_b200 import capi
+
+    w, h = 16, 8
+    g = capi.GrbGBuffer()
+    keep = [np.zeros((h, w), np.uint32), np.zeros((h, w), np.uint32), np.zeros((h, w), np.uint16), np.zeros((h, w), np.float32)]
+    g.albedo = _image(capi, keep[0], capi.FORMAT_R8G8B8A8_SRGB)
+    g.normal = _image(capi, keep[1], capi.FORMAT_A2B10G10R10_UNORM)
+    g.pbr = _image(capi, keep[2], capi.FORMAT_R8G8_UNORM)
+    g.depth = _image(capi, keep[3], capi.FORMAT_D32_SFLOAT)
+    hdr = _image(capi, np.zeros((h, w), np.uint32), capi.FORMAT_B10G11R11_UFLOAT)
+    cam, params, bufs = capi.GrbCamera(), capi.GrbClusterParameters(), capi.GrbClusterBuffers()
+    params.num_lights, params.num_lights_32 = 4, 1
+    table = np.zeros(64, np.uint32)
+    base = (table.ctypes.data + 15) // 16 * 16
+    bufs.type_mask = bufs.bitmask = bufs.cluster_range = base
+    rows = capi.GrbRows(0, 0)
+    cost = np.zeros(4, np.uint32)
+    for off in (4, 8, 12):
+        bufs.lights = base + off
+        assert lib.grb_deferred_lighting(C.byref(g), C.byref(cam), C.byref(params), C.byref(bufs), C.byref(hdr), rows, None) == ERR_ARG
+        assert "16-byte" in _msg(lib)
+        assert lib.grb_deferred_lighting_blocks(C.byref(g), C.byref(cam), C.byref(params), C.byref(bufs), C.byref(hdr), rows, None) == ERR_ARG
+        assert lib.grb_deferred_lighting_scheduled(C.byref(g), C.byref(cam), C.byref(params), C.byref(bufs), C.byref(hdr), rows, None, None) == ERR_ARG
+        assert lib.grb_lighting_row_cost(C.byref(g.depth), C.byref(cam), C.byref(params), C.byref(bufs), rows,
+                                         cost.ctypes.data_as(C.c_void_p), None) == ERR_ARG
+        assert "16-byte" in _msg(lib)
+    assert cost.sum() == 0

@@ -10,10 +10,8 @@ GETENV = re.compile(r'getenv\(\s*"(GRB_[A-Z0-9_]+)"\s*\)')
 
 ALLOWED_UNTESTED = {
     "GRB_HOST_PROFILE": "prints host-side timings only; no computed value depends on it",
-    "GRB_LIGHTING_V2": "lighting pairs form: its bar needs its own argument (sums associate differently); a follow-up covers it",
-    "GRB_LIGHTING_1PX": "lighting one-pixel form: its bar needs its own argument (sums associate differently); a follow-up covers it",
-    "GRB_LIGHTING_ROW_BLOCKS": "block size of the lighting pairs form; covered with that form in a follow-up",
-    "GRB_SHARDED_BLOCKS": "lighting block form on row-sharded frames; covered with the lighting forms in a follow-up",
+    "GRB_SHARDED_BLOCKS": "selects grb_deferred_lighting_blocks for row-sharded frames; that form is tested on row bands in "
+                          "test_zo_gpu_lighting_forms.py, the switch itself needs a multi-rank run not written yet",
 }
 
 
