@@ -20,6 +20,7 @@ struct NcclUniqueId
 using ncclComm_t = void *;
 constexpr int ncclSuccess = 0;
 constexpr int ncclInt8 = 0;   // ncclChar
+constexpr int ncclUint32 = 3;
 constexpr int ncclFloat32 = 7; // ncclFloat
 constexpr int ncclSum = 0;
 
@@ -175,6 +176,15 @@ bool NcclCollectives::all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, si
 	if (nccl_ok(api().AllReduce(data, data, count, ncclFloat32, ncclSum, comm, cmd.get_stream_handle()), "ncclAllReduce"))
 		return true;
 	return collective_failed("all_reduce_sum");
+}
+
+bool NcclCollectives::all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, size_t count)
+{
+	if (!comm)
+		return false;
+	if (nccl_ok(api().AllReduce(data, data, count, ncclUint32, ncclSum, comm, stream), "ncclAllReduce"))
+		return true;
+	return collective_failed("all_reduce_sum_u32");
 }
 
 // ----------------------------------------------------------------------------- peer exchange

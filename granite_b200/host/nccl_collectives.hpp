@@ -25,6 +25,7 @@ public:
 	unsigned get_world_size() const override { return world; }
 	bool all_gather_rows(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<GrbRows> &rows) override;
 	bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) override;
+	bool all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, size_t count) override;
 	// Peer-memory exchange: two image slots + a flag array per rank, cudaIpc-mapped into every
 	// other rank (handles are exchanged with one ncclAllGather).  GRB_SHARD_EXCHANGE=nccl disables it.
 	bool peer_exchange_begin_frame(PeerChannel channel, size_t image_bytes, PeerSlot &slot) override;

@@ -810,6 +810,14 @@ void RenderGraph::set_row_shards(const std::vector<GrbRows> &bands, unsigned ran
 	collectives = collectives_;
 }
 
+void RenderGraph::move_row_shards(const std::vector<GrbRows> &bands)
+{
+	if (shard_bands.size() <= 1 || bands.size() != shard_bands.size())
+		throw std::logic_error("move_row_shards: a sharded graph keeps its band count.");
+	check_band_layout(swapchain_dimensions.width, swapchain_dimensions.height, bands, shard_upscale);
+	shard_bands = bands;
+}
+
 GrbRows RenderGraph::shard_rows_for_rank(unsigned rank, unsigned resource_height, unsigned halo_rows) const
 {
 	GrbRows r = { 0, 0 };

@@ -49,6 +49,15 @@ public:
 	// Every rank contributes rows [rows[r].y0, rows[r].y1) of an image all ranks hold at full size.
 	virtual bool all_gather_rows(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<GrbRows> &rows) = 0;
 	virtual bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) = 0;
+	// Exact integer sum over ranks (modulo 2^32), in place on `stream`; false = not available.  For small host-driven
+	// reductions outside the graph (the viewer's sharded row-cost measurement).
+	virtual bool all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, size_t count)
+	{
+		(void)stream;
+		(void)data;
+		(void)count;
+		return false;
+	}
 
 	// Peer-memory exchange: a double-buffered image every rank holds in full, of which each rank
 	// PRODUCES some rows per frame by storing them into all ranks' copies from its own kernel
@@ -480,6 +489,11 @@ public:
 	// stay backbuffer rows; every stage before FSR gets render rows).
 	void set_row_shards(const std::vector<GrbRows> &bands, unsigned rank, RenderGraphCollectives *collectives, bool fxaa_downstream = false,
 	                    int smaa_quality_downstream = -1, bool taa_upstream = false, ShardUpscale upscale = {});
+	// Moves the band cuts of a sharded graph between two frames: replaces the bands only (same count, same rank, same
+	// collectives and options).  Every pass reads its rows from get_shard_plan() when it records, so the next frame
+	// runs on the new cuts without a re-bake; attachments, histories and peer channels stay (DESIGN.md section 5,
+	// "Moving the bands between frames").
+	void move_row_shards(const std::vector<GrbRows> &bands);
 	// Rows of every stage for `rank` (this rank by default); whole images when unsharded.
 	ShardPlan get_shard_plan() const { return get_shard_plan(shard_rank); }
 	ShardPlan get_shard_plan(unsigned rank) const

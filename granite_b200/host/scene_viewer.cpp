@@ -62,6 +62,9 @@ struct GrbhViewer
 	// `presented` is where this frame's whole image lies on that rank (the channel's slot, or the gathered output)
 	int present_rank = -1;
 	const void *presented = nullptr;
+	// grbh_viewer_move_row_shards ran since the last frame: the resident G-buffer, the last output and the last depth
+	// image hold the old layout's rows until a frame (which must bring the host G-buffer) renders on the new one
+	bool bands_moved = false;
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
@@ -134,6 +137,7 @@ struct GrbhViewer
 
 	void bake_render_graph();
 	void render_frame(const GrbhHostGBuffer *host, double frame_time);
+	int32_t measure_row_cost_sharded(uint32_t *out, int groups);
 };
 
 void GrbhViewer::bake_render_graph()
@@ -418,6 +422,8 @@ void GrbhViewer::bake_render_graph()
 
 cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
 {
+	if (bands_moved)
+		throw std::runtime_error("output readback: the bands moved (grbh_viewer_move_row_shards) since the last frame; render a frame first");
 	auto &output = graph.get_texture_resource(output_name);
 	const void *base = graph.get_physical_texture_resource(output).get_image().get_device_pointer();
 	r = bands.size() > 1 ? bands[rank] : GrbRows{ 0, config.height };
@@ -435,6 +441,46 @@ cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
 	                     "output readback"))
 		throw std::runtime_error("cudaMemcpyAsync failed");
 	return stream;
+}
+
+// The row cost of a row-sharded frame: each rank measures the rows it produced (its band, or its render rows under
+// FSR 1), whose depth it holds and whose cluster tiles it binned, into a zero-filled whole-frame vector; an integer
+// all-reduce then sums the ranks' disjoint pieces.  The kernel charges each 4-row group for its own pixels only and
+// sums with integer atomics, so with every cut on a multiple of 4 rows the result is the unsharded viewer's, bit for
+// bit.  Collective: every rank calls it after the same frame.
+int32_t GrbhViewer::measure_row_cost_sharded(uint32_t *out, int groups)
+{
+	if (bands_moved)
+		return fail("grbh_viewer_measure_row_cost: the bands moved (grbh_viewer_move_row_shards) since the last frame; render a frame first");
+	for (const GrbRows &r : graph.get_shard_plan_rows(&ShardPlan::render_own))
+		if (r.y0 % 4 != 0)
+			return fail("grbh_viewer_measure_row_cost: a row-sharded measurement needs every cut on a multiple of 4 rows (render row " +
+			            std::to_string(r.y0) + ")");
+	RenderGraphCollectives *coll = graph.get_collectives();
+	device->wait_idle();
+	const GrbRows rows = shard_plan().render_own;
+	GrbImage depth = graph.get_physical_texture_resource(*res_depth).as_grb();
+	GrbCamera cam;
+	if (grbh_viewer_get_camera(this, &cam, nullptr, nullptr) != 0)
+		return -1;
+	GrbClusterParameters params = cluster.get_cluster_parameters_bindless();
+	GrbClusterBuffers buffers = cluster.get_cluster_buffers();
+	auto stream = reinterpret_cast<cudaStream_t>(device->get_stream());
+	uint32_t *dev = nullptr;
+	if (!Vulkan::cuda_ok(cudaMalloc(&dev, sizeof(uint32_t) * groups), "cudaMalloc"))
+		return fail("cudaMalloc failed");
+	bool ok = Vulkan::cuda_ok(cudaMemsetAsync(dev, 0, sizeof(uint32_t) * groups, stream), "cudaMemsetAsync");
+	const int32_t rc = ok ? grb_lighting_row_cost(&depth, &cam, &params, &buffers, rows, dev + rows.y0 / 4, stream) : GRB_OK;
+	const std::string kernel_error = rc != GRB_OK ? grb_last_error_string() : "";
+	// every rank joins the reduction, also one whose own part failed, so that no peer waits in it alone
+	const bool reduced = coll && coll->all_reduce_sum_u32(stream, dev, (size_t)groups);
+	const bool synced = Vulkan::cuda_ok(cudaStreamSynchronize(stream), "cudaStreamSynchronize");
+	ok = ok && rc == GRB_OK && reduced && synced && Vulkan::cuda_ok(cudaMemcpy(out, dev, sizeof(uint32_t) * groups, cudaMemcpyDeviceToHost), "cudaMemcpy");
+	cudaFree(dev);
+	if (!ok)
+		return fail(!kernel_error.empty() ? kernel_error
+		                                  : (reduced ? "grbh_viewer_measure_row_cost: copy failed" : "grbh_viewer_measure_row_cost: the all-reduce over the ranks failed"));
+	return groups;
 }
 
 void GrbhViewer::render_frame(const GrbhHostGBuffer *host, double frame_time)
@@ -760,6 +806,39 @@ extern "C" int32_t grbh_viewer_set_present_rank(GrbhViewer *v, int32_t rank)
 	return 0;
 }
 
+extern "C" int32_t grbh_viewer_move_row_shards(GrbhViewer *v, const GrbRows *bands, int32_t count)
+{
+	if (!v || !bands || count <= 0)
+		return fail("grbh_viewer_move_row_shards: bad arguments");
+	if (v->bands.size() <= 1)
+		return fail("grbh_viewer_move_row_shards: the viewer is not row-sharded (grbh_viewer_set_row_shards with more than one band)");
+	if ((size_t)count != v->bands.size())
+		return fail("grbh_viewer_move_row_shards: " + std::to_string(count) + " bands for a viewer of " + std::to_string(v->bands.size()) +
+		            " (the band count of a viewer is fixed; re-bake to change it)");
+	GRBH_TRY
+	// the checks that need no device come first, so that a host-only viewer reaches them
+	const std::vector<GrbRows> moved(bands, bands + count);
+	try
+	{
+		// under FSR 1 every rank must also produce render rows for the exchanges (shard_plan.hpp)
+		check_band_layout((unsigned)v->config.width, (unsigned)v->config.height, moved, v->shard_upscale());
+	}
+	catch (const std::invalid_argument &e)
+	{
+		return fail(std::string("grbh_viewer_move_row_shards: ") + e.what());
+	}
+	// the band count and the rank stay, so the presenting rank (< the band count) keeps its band
+	if (!v->baked)
+		return fail("grbh_viewer_move_row_shards: viewer not baked (before bake, grbh_viewer_set_row_shards sets the bands)");
+	v->graph.move_row_shards(moved); // the graph's bands only: no reset, no bake, no allocation, same collectives
+	v->bands = moved;
+	const GrbRows lit = v->input_rows();
+	v->cluster.set_lit_pixel_rows(lit.y0, lit.y1, v->render_height());
+	v->bands_moved = true;
+	return 0;
+	GRBH_CATCH
+}
+
 extern "C" int32_t grbh_shard_plan(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t fxaa, GrbRows *out9)
 {
 	if (width <= 0 || height <= 0 || count < 0 || (count && !bands) || !out9 || (count && (rank < 0 || rank >= count)))
@@ -860,9 +939,14 @@ extern "C" int32_t grbh_viewer_render_frame(GrbhViewer *v, const GrbhHostGBuffer
 		return fail("grbh_viewer_render_frame: viewer not baked");
 	if (v->config.pipelined_io && !host)
 		return fail("grbh_viewer_render_frame: pipelined_io viewers need the host G-buffer every frame");
+	if (v->bands_moved && (!host || (v->uses_taa() && !host->mv)))
+		return fail(std::string("grbh_viewer_render_frame: the bands moved (grbh_viewer_move_row_shards) since the last frame and the resident "
+		                        "G-buffer holds the old rows; this frame must bring the host G-buffer") +
+		            (v->uses_taa() ? " with its motion vectors" : ""));
 	GRBH_TRY
 	cudaSetDevice(v->device->get_device_index());
 	v->render_frame(host, frame_time);
+	v->bands_moved = false;
 	return 0;
 	GRBH_CATCH
 }
@@ -1120,12 +1204,13 @@ extern "C" int32_t grbh_viewer_measure_row_cost(GrbhViewer *v, uint32_t *out, in
 {
 	if (!v || !v->baked || !v->device || !out)
 		return fail("grbh_viewer_measure_row_cost: needs a baked device viewer");
-	if (v->graph.is_sharded())
-		return fail("grbh_viewer_measure_row_cost: the viewer must hold the whole frame (not row-sharded)");
 	GRBH_TRY
 	const int groups = (v->render_height() + 3) / 4;
 	if (capacity < groups)
 		return fail("grbh_viewer_measure_row_cost: capacity too small");
+	const bool sharded = v->graph.is_sharded() && v->graph.get_shard_count() > 1;
+	if (sharded)
+		return v->measure_row_cost_sharded(out, groups);
 	v->device->wait_idle();
 	GrbImage depth = v->graph.get_physical_texture_resource(*v->res_depth).as_grb();
 	GrbCamera cam;

@@ -139,4 +139,19 @@ ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<
 	p.lum_grid.y1 = rank + 1 < bands.size() ? begin_of(rank + 1) : (int)h_grid;
 	return p;
 }
+
+void check_band_layout(unsigned width, unsigned height, const std::vector<GrbRows> &bands, ShardUpscale upscale)
+{
+	int expect = 0;
+	for (const GrbRows &b : bands)
+	{
+		if (b.y0 != expect || b.y1 <= b.y0)
+			throw std::invalid_argument("the bands must tile the frame in order");
+		expect = b.y1;
+	}
+	if (expect != (int)height)
+		throw std::invalid_argument("the bands must cover rows [0, " + std::to_string(height) + ")");
+	if (upscale.height && bands.size() > 1)
+		compute_shard_plan(width, height, bands, 0, false, -1, false, upscale); // throws when a rank would produce no render rows
+}
 } // namespace Granite

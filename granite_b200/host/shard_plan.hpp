@@ -112,4 +112,8 @@ struct ShardUpscale
 // (render_own) would be empty.
 ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1,
                              bool taa = false, ShardUpscale upscale = {});
+
+// A new layout for moving the cuts of a sharded frame: throws std::invalid_argument unless `bands` tile [0, height) in
+// order, or (under FSR 1) when a rank would produce no render rows.
+void check_band_layout(unsigned width, unsigned height, const std::vector<GrbRows> &bands, ShardUpscale upscale);
 } // namespace Granite

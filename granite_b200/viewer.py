@@ -382,6 +382,14 @@ class Viewer:
         frame.  Every rank sets the same value, before bake."""
         _check(lib().grbh_viewer_set_present_rank(self._h, int(rank)), "grbh_viewer_set_present_rank")
 
+    def move_row_shards(self, bands):
+        """Move the band cuts of a baked row-sharded viewer from the next frame on, without a re-bake: the TAA history,
+        bloom feedback and every attachment carry over.  Same band count; the bands tile [0, height).  The next
+        render_frame must bring the host G-buffer (with motion vectors under TAA).  Collective: every rank passes the
+        same bands between the same two frames (grbh_viewer_move_row_shards)."""
+        arr = (capi.GrbRows * max(len(bands), 1))(*[capi.GrbRows(a, b) for a, b in bands])
+        _check(lib().grbh_viewer_move_row_shards(self._h, arr, len(bands)), "grbh_viewer_move_row_shards")
+
     def bake(self):
         _check(lib().grbh_viewer_bake(self._h), "grbh_viewer_bake")
 
@@ -489,12 +497,13 @@ class Viewer:
         return out.reshape(4, 4)
 
     def measure_row_cost(self) -> np.ndarray:
-        """Estimated lighting work (warp instructions) per group of 4 rows of the frame rendered last;
-        unsharded viewers only (grbh_viewer_measure_row_cost)."""
-        groups = (self.height + 3) // 4
+        """Estimated lighting work (warp instructions) per group of 4 rows of the render-size image of the frame
+        rendered last (grbh_viewer_measure_row_cost).  On a row-sharded viewer this is collective: every rank calls it
+        after the same frame and gets the same whole-frame vector, the one an unsharded viewer returns."""
+        groups = (self.render_size()[1] + 3) // 4
         out = np.zeros(groups, np.uint32)
-        _check(lib().grbh_viewer_measure_row_cost(self._h, _vp(out), groups), "grbh_viewer_measure_row_cost")
-        return out
+        n = _check(lib().grbh_viewer_measure_row_cost(self._h, _vp(out), groups), "grbh_viewer_measure_row_cost")
+        return out[:n]
 
     def pass_names(self):
         buf = C.create_string_buffer(4096)

@@ -125,7 +125,8 @@ int32_t grbh_load_gtx(const char *path, int32_t *format, int32_t *width, int32_t
  * primaries_xy8: red, green, blue, white chromaticities (VkHdrMetadataEXT order); out16: column-major mat4. */
 int32_t grbh_rec709_to_display_primaries(const float *primaries_xy8, float *out16);
 
-/* Row sharding (multi-GPU): bands[r] = backbuffer rows of rank r.  Must precede bake.  With FSR 1 upscaling, a layout in
+/* Row sharding (multi-GPU): bands[r] = backbuffer rows of rank r.  Must precede bake (a baked viewer moves its cuts with
+ * grbh_viewer_move_row_shards below).  With FSR 1 upscaling, a layout in
  * which some rank would produce no render rows (grbh_shard_plan_fsr) is refused, and so is a layout with fewer bands
  * than the presenting rank of grbh_viewer_set_present_rank needs. */
 int32_t grbh_nccl_unique_id(uint8_t out128[128]);
@@ -139,11 +140,30 @@ int32_t grbh_viewer_set_row_shards(GrbhViewer *viewer, const GrbRows *bands, int
  * Every rank must set the same value.  Must precede bake.  Readers of the presented frame must be stream-ordered
  * behind the frame (these readbacks are): DESIGN.md section 5, "Presenting a sharded frame". */
 int32_t grbh_viewer_set_present_rank(GrbhViewer *viewer, int32_t rank);
+/* Moves the band cuts of a baked row-sharded viewer; takes effect from the next grbh_viewer_render_frame.
+ * bands: `count` rows ranges that tile [0, height) in order, count = the band count the viewer was baked with; the rank
+ * stays.  Under FSR 1 a layout in which some rank would produce no render rows is refused, as by
+ * grbh_viewer_set_row_shards.  A refused layout returns an error and leaves the viewer as it was.  Nothing is re-baked
+ * or allocated: attachments, the TAA history, the bloom feedback, the average luminance, the lighting schedule and the
+ * peer channels carry over, and the next frame is the one an unsharded viewer renders (DESIGN.md section 5, "Moving the
+ * bands between frames"; with FXAA and no upscale, bit-exact only for cuts on multiples of 16 rows).
+ * The resident G-buffer holds the old layout's rows, so the first grbh_viewer_render_frame after a move must bring the
+ * host G-buffer (with its motion vectors under TAA): a NULL one is refused there, and so are output readbacks and
+ * grbh_viewer_measure_row_cost until that frame has been rendered.  Readbacks enqueued before the move keep the rows
+ * they reported.
+ * Collective contract: every rank calls it with the same bands, between the same two grbh_viewer_render_frame calls
+ * (the checks give every rank the same answer for the same input).  Ranks that disagree on the layout run mismatched
+ * exchanges. */
+int32_t grbh_viewer_move_row_shards(GrbhViewer *viewer, const GrbRows *bands, int32_t count);
 
-/* Work estimate of the lighting pass per group of 4 backbuffer rows for the frame last rendered by
- * an UNSHARDED viewer (its depth image and light cluster are resident): grb_lighting_row_cost() on
- * the viewer's resources, copied to the host.  out: ceil(height / 4) values.  Feed the sums per
- * band unit to a weighted partition to get bands of equal lighting work (granite_b200/viewer.py). */
+/* Work estimate of the lighting pass per group of 4 rows of the render-size image (the backbuffer without FSR 1) for
+ * the frame last rendered: grb_lighting_row_cost() on the viewer's depth image and light cluster, copied to the host.
+ * out: ceil(render height / 4) values; returns that count.  Feed the sums per band unit to a weighted partition to
+ * get bands of equal lighting work (granite_b200/viewer.py: band_partition_measured).
+ * A row-sharded viewer measures on each rank the rows it produced (its band, or its render rows under FSR 1) and sums
+ * the ranks' pieces with an exact integer all-reduce over its collectives: every rank returns the same whole-frame
+ * vector, equal bit for bit to the unsharded viewer's.  That form is collective (every rank calls it after the same
+ * frame) and needs every cut on a multiple of 4 rows. */
 int32_t grbh_viewer_measure_row_cost(GrbhViewer *viewer, uint32_t *out, int32_t capacity);
 
 /* The row plan of one rank of a row-sharded frame (granite_b200/host/shard_plan.hpp): out8 =
