@@ -1,9 +1,16 @@
 """Shared helpers for the parity tests (test infrastructure)."""
 from __future__ import annotations
 
+import os
+import signal
+import subprocess
+import sys
+
 import numpy as np
 
 from granite_b200 import synth
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def free_port() -> int:
@@ -14,6 +21,26 @@ def free_port() -> int:
     with socket.socket() as s:
         s.bind(("", 0))
         return s.getsockname()[1]
+
+
+def run_ranks(worker, args, world, env, timeout):
+    """Run tests/<worker> on `world` ranks under torchrun, with `env` added to the environment; returns (returncode,
+    stdout, stderr).  The launcher runs in a session of its own, so that a run past `timeout` seconds is killed with
+    every rank it started, and the test fails."""
+    import pytest
+
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
+           "--master-port", str(free_port()), os.path.join(ROOT, "tests", worker), *map(str, args)]
+    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=dict(os.environ, **env),
+                            start_new_session=True)
+    try:
+        out, err = proc.communicate(timeout=timeout)
+    except subprocess.TimeoutExpired:
+        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
+        out, err = proc.communicate()
+        pytest.fail(f"the sharded run did not finish in {timeout} s:\n" + out[-3000:] + err[-3000:])
+    sys.stdout.write(out[-6000:])
+    return proc.returncode, out, err
 
 
 def build_case(oracle, width, height, n_lights, spot_fraction=0.0):

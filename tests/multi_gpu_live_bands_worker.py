@@ -18,8 +18,10 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from granite_b200 import synth, viewer  # noqa: E402
+from tests import sharded  # noqa: E402
 
 FRAMES = 8
 MOVES = (3, 6)  # frames rendered first on a new layout
@@ -29,25 +31,8 @@ RUNS = (("no AA", None, True, "fixed"), ("FXAA", None, False, "fixed"), ("SMAA U
         ("TAA High + FXAA", -1, False, "fixed"), ("no AA", None, True, "measured"))
 
 
-def config_args(name):
-    from granite_b200 import viewer
-
-    return {"no AA": dict(post_aa=viewer.AA_NONE), "FXAA": dict(post_aa=viewer.AA_FXAA), "SMAA Ultra": dict(post_aa=viewer.AA_SMAA_ULTRA),
-            "TAA High + FXAA": dict(post_aa=viewer.AA_TAA_HIGH_PLUS_FXAA), "FSR 0.67 + RCAS": dict(resolution_scale=0.67, resolution_scale_sharpen=True),
-            "HDR10 + TAA": dict(post_aa=viewer.AA_TAA_HIGH, hdr10_output=True)}[name]
-
-
 def uses_taa(name):
     return "TAA" in name
-
-
-def motion_vectors(w, h):
-    rng = np.random.default_rng(5)
-    mv = np.zeros((h, w, 2), np.float16)
-    moving = rng.random((h, w)) < 0.15
-    n = int(moving.sum())
-    mv[moving] = np.stack([rng.uniform(-4.0, 4.0, n) / w, rng.uniform(-0.5, 0.5, n)], -1).astype(np.float16)
-    return mv
 
 
 def expect_refusal(fn, what):
@@ -61,24 +46,8 @@ def expect_refusal(fn, what):
 
 def main():
     w, h, n_lights = int(sys.argv[1]), int(sys.argv[2]), int(sys.argv[3])
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    gpus = torch.cuda.device_count()
-    if world > gpus:
-        # ranks share a device: each names a host of its own so that NCCL accepts them (see multi_gpu_worker.py)
-        os.environ["NCCL_HOSTID"] = f"granite-test-rank-{rank}"
-        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
-        os.environ.setdefault("NCCL_IB_DISABLE", "1")
-    local = local % gpus
-    torch.cuda.set_device(local)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    from granite_b200 import synth, viewer
-
-    luts = np.load(os.path.join(ROOT, "tests", "golden", "refsmaa_160x96.npz"))
-    scene = synth.make_scene(w, h)
-    lights = synth.make_lights(n_lights, spot_fraction=0.25, aspect=w / h)
-    keep = [np.ascontiguousarray(a) for a in (scene.albedo, scene.normal, scene.pbr, scene.depth, scene.emissive)]
-    keep.append(np.ascontiguousarray(motion_vectors(w, h)).view(np.uint32).reshape(h, w))
-    gb = viewer.Viewer.host_gbuffer(*keep)
+    rank, world, _ = sharded.init_ranks()
+    scene, lights, keep, gb = sharded.inputs(w, h, n_lights, mv=sharded.motion_vectors(w, h, 5))
     gb_no_mv = viewer.Viewer.host_gbuffer(*keep[:5])
     views = [synth.look_at_view((0.15 * i, 0.1 * i, 8.0 - 0.2 * i), (0.0, 0.0, 0.0)) for i in range(FRAMES)]
     equal = viewer.band_partition(h, world)
@@ -93,24 +62,6 @@ def main():
         narrow.append((y0, h if r == world - 1 else y0 + 16 * max(rest // (world - 2), 1)))
     fixed_layouts = {0: equal, MOVES[0]: shifted, MOVES[1]: narrow}
 
-    def make(cfg, bands, present_rank=None):
-        v = viewer.Viewer(w, h, cuda_device=local, **config_args(cfg))
-        v.set_directional(scene.dir_color, scene.dir_direction)
-        v.set_lights(lights)
-        v.set_smaa_lookup_textures(luts["area"], luts["search"])
-        if bands:
-            uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
-            if rank == 0:
-                uid.copy_(torch.frombuffer(bytearray(viewer.nccl_unique_id()), dtype=torch.uint8))
-            dist.broadcast(uid, 0)
-            v.init_collectives(uid.cpu().numpy().tobytes(), rank, world)
-            v.set_row_shards(bands, rank)
-            if present_rank is not None:
-                v.set_present_rank(present_rank)
-        v.set_camera(scene.projection, views[0])
-        v.bake()
-        return v
-
     ok = True
     references = {}
     for cfg, present, measure, layouts in RUNS:
@@ -118,12 +69,8 @@ def main():
             # the unsharded frames (and row costs) on rank 0, shared with every rank
             frames, costs = [], []
             if rank == 0:
-                v1 = make(cfg, None)
-                for i in range(FRAMES):
-                    v1.set_camera(scene.projection, views[i])
-                    v1.render_frame(gb if i == 0 else None)
-                    ref = np.zeros((h, w), np.uint32)
-                    v1.read_output(ref)
+                v1 = sharded.make_viewer(w, h, scene, lights, views[0], **sharded.config_args(cfg))
+                for ref, _ in sharded.frames(v1, gb, scene.projection, views):
                     frames.append(ref)
                     costs.append(v1.measure_row_cost())
                 v1.close()
@@ -134,7 +81,7 @@ def main():
 
         p = None if present is None else present % world
         bands = equal
-        vs = make(cfg, bands, p)
+        vs = sharded.make_viewer(w, h, scene, lights, views[0], bands, p, **sharded.config_args(cfg))
         label = f"{cfg} {layouts}{'' if p is None else f' P={p}'}"
         for i in range(FRAMES):
             if i in MOVES:
@@ -160,16 +107,10 @@ def main():
             vs.render_frame(gb if i == 0 or i in MOVES else None)
             out = np.zeros((h, w), np.uint32)
             rows = vs.read_output(out)
-            if p is None:
-                ok &= rows == tuple(bands[rank])
-                full = torch.from_numpy(out.view(np.int32)).cuda()
-                dist.all_reduce(full, op=dist.ReduceOp.SUM)  # bands are disjoint, zeros elsewhere
-            else:
-                ok &= rows == ((0, h) if rank == p else tuple(bands[rank]))
-                full = torch.from_numpy(out.view(np.int32)).cuda()
-                dist.broadcast(full, p)
+            ok &= rows == ((0, h) if rank == p else tuple(bands[rank]))
+            full = sharded.assemble(out, p)
             if rank == 0:
-                same = np.array_equal(full.cpu().numpy().view(np.uint32), reference[i])
+                same = np.array_equal(full, reference[i])
                 print(f"{label} frame {i} bands {bands}: live bands == single GPU: {same}", flush=True)
                 ok &= same
             if measure and layouts == "fixed" and i in (1, MOVES[0] + 1, MOVES[1] + 1):
@@ -179,15 +120,8 @@ def main():
                 if rank == 0:
                     print(f"{label} frame {i}: sharded row cost == single GPU on every rank: {bool(same.item())}", flush=True)
                 ok &= bool(same.item())
-        # every rank's pushes and flag stores have landed before any rank frees its channels
-        vs.sync()
-        dist.barrier()
-        vs.close()
-
-    flag = torch.tensor([1 if ok else 0], device="cuda")
-    dist.all_reduce(flag, op=dist.ReduceOp.MIN)
-    dist.destroy_process_group()
-    sys.exit(0 if int(flag.item()) == 1 else 1)
+        sharded.close_sharded(vs)
+    sharded.finish(ok)
 
 
 if __name__ == "__main__":

@@ -1,33 +1,11 @@
 """Row-sharded viewers whose band cuts move between frames without a re-bake (grbh_viewer_move_row_shards), and the
 sharded row-cost measurement, against the unsharded viewer with both exchange paths of the C++ graph (peer-memory
 stores, NCCL).  The worker is tests/multi_gpu_live_bands_worker.py."""
-import os
-import signal
-import subprocess
-import sys
-
 import pytest
 
 from tests import common
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _run_worker(exchange, port):
-    world = 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multi_gpu_live_bands_worker.py"), "640", "384", "200"]
-    env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
-    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
-    try:
-        out, err = proc.communicate(timeout=1200)
-    except subprocess.TimeoutExpired:
-        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
-        out, err = proc.communicate()
-        pytest.fail("the sharded run did not finish in 1200 s:\n" + out[-3000:] + err[-3000:])
-    sys.stdout.write(out[-6000:])
-    return proc.returncode, out, err
 
 
 @pytest.mark.parametrize("exchange", ["peer", "nccl"])
@@ -38,7 +16,7 @@ def test_moved_bands_keep_frames_bit_identical(cuda, exchange):
     sharded row cost equals the unsharded one on every rank, and the bands cut from it agree on every rank."""
     from tests.multi_gpu_live_bands_worker import FRAMES, RUNS
 
-    rc, out, err = _run_worker(exchange, common.free_port())
+    rc, out, err = common.run_ranks("multi_gpu_live_bands_worker.py", [640, 384, 200], 4, {"GRB_SHARD_EXCHANGE": exchange}, 1200)
     assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count("live bands == single GPU: True") == len(RUNS) * FRAMES, out[-3000:]
     assert "live bands == single GPU: False" not in out

@@ -1,18 +1,12 @@
 """Presenting row-sharded frames from one rank on the GPU: the kernel that pushes a rank's band of the final image into
 the presenting rank's frame slot (grb_present_rows_to_peer), and whole sharded frames read on the presenting rank
 against the unsharded frame with both exchange paths of the C++ graph (peer-memory stores, NCCL all-gather)."""
-import os
-import signal
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
 from tests import common
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SENTINEL = 0x3C3C3C3C
 
 
@@ -50,22 +44,6 @@ def test_present_kernel_routes_own_rows(cuda, width, image_width):
     assert not counters[0].item() and not counters[1].item()  # the last CTA resets the scratch counter
 
 
-def _run_worker(exchange, port):
-    world = 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(ROOT, "tests", "multi_gpu_present_worker.py"), "640", "384", "200"]
-    env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
-    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
-    try:
-        out, err = proc.communicate(timeout=1200)
-    except subprocess.TimeoutExpired:
-        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
-        out, err = proc.communicate()
-        pytest.fail("the sharded run did not finish in 1200 s:\n" + out[-3000:] + err[-3000:])
-    sys.stdout.write(out[-6000:])
-    return proc.returncode, out, err
-
-
 @pytest.mark.parametrize("exchange", ["peer", "nccl"])
 def test_presented_sharded_frame_is_bit_identical(cuda, exchange):
     """4 ranks (sharing GPUs where there are fewer); no AA, FXAA, SMAA Ultra, TAA High + FXAA, FSR 0.67 + RCAS, HDR10 +
@@ -74,7 +52,7 @@ def test_presented_sharded_frame_is_bit_identical(cuda, exchange):
     unsharded frame, and the other ranks return their bands."""
     from tests.multi_gpu_present_worker import CONFIGS, FRAMES, RUNS
 
-    rc, out, err = _run_worker(exchange, common.free_port())
+    rc, out, err = common.run_ranks("multi_gpu_present_worker.py", [640, 384, 200], 4, {"GRB_SHARD_EXCHANGE": exchange}, 1200)
     assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count("tonemap-only sharded == single GPU: True") == 2 * FRAMES, out[-3000:]
     assert out.count("presented == single GPU: True") == len(CONFIGS) * len(RUNS) * FRAMES, out[-3000:]

@@ -1,17 +1,11 @@
 """FSR 1 upscaling on row-sharded frames on the GPU: whole sharded frames against the unsharded frame with both exchange
 paths of the C++ graph (peer-memory stores, NCCL all-gathers), the render rows of every pass before FSR taken from
 grbh_shard_plan_fsr."""
-import os
-import signal
-import subprocess
-import sys
-
 import pytest
 
 from tests import common
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CONFIGS = 6
 
 
@@ -21,18 +15,8 @@ def test_sharded_fsr_frame_is_bit_identical(cuda, exchange):
     High + FXAA, 0.67 without RCAS and SMAA Ultra, 0.5 with RCAS and SMAA Low, 0.5 without RCAS and TAA Low; equal and
     narrow bands; 4 frames each."""
     world = 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_fsr_worker.py"), "1280", "768", "300"]
-    env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
-    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
-    try:
-        out, err = proc.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
-        out, err = proc.communicate()
-        pytest.fail("the sharded run did not finish in 900 s:\n" + out[-3000:] + err[-3000:])
-    sys.stdout.write(out[-4000:])
-    assert proc.returncode == 0, out[-3000:] + err[-3000:]
+    rc, out, err = common.run_ranks("multi_gpu_fsr_worker.py", [1280, 768, 300], world, {"GRB_SHARD_EXCHANGE": exchange}, 900)
+    assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count(f"sharded over {world} ranks == single GPU: True") == CONFIGS * 2 * 4, out[-3000:]
     if exchange == "peer":
         assert "peer-memory exchange unavailable" not in out + err, "IPC works between the ranks: the peer path must be the one that ran"

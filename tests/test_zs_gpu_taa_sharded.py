@@ -1,18 +1,12 @@
 """TAA on row-sharded frames on the GPU: the resolve kernel that stores its own history rows into every rank's history
 image (grb_taa_resolve_to_peers), and whole sharded frames against the unsharded frame with both exchange paths of the
 C++ graph (peer-memory stores, NCCL all-gather)."""
-import os
-import signal
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
 from tests import common
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SENTINEL16 = 0x5A5A
 SENTINEL32 = 0x3C3C3C3C
 
@@ -78,18 +72,8 @@ def test_sharded_taa_frame_is_bit_identical(cuda, exchange):
     """4 ranks (sharing GPUs where there are fewer); TAA Low, High, High + FXAA, High with HDR10 output; equal and
     narrow bands; 6 frames each with a moving camera and large vertical motion vectors."""
     world = 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_taa_worker.py"), "1280", "768", "300"]
-    env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
-    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
-    try:
-        out, err = proc.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
-        out, err = proc.communicate()
-        pytest.fail("the sharded run did not finish in 900 s:\n" + out[-3000:] + err[-3000:])
-    sys.stdout.write(out[-4000:])
-    assert proc.returncode == 0, out[-3000:] + err[-3000:]
+    rc, out, err = common.run_ranks("multi_gpu_taa_worker.py", [1280, 768, 300], world, {"GRB_SHARD_EXCHANGE": exchange}, 900)
+    assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count(f"sharded over {world} ranks == single GPU: True") == 4 * 2 * 6, out[-3000:]
     assert out.count("motion vectors reach other bands from every rank: True") == 2, out[-3000:]
     if exchange == "peer":

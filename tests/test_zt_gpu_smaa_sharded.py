@@ -1,11 +1,6 @@
 """SMAA on row-sharded frames on the GPU: the edge kernel that stores its rows into the peers' edge images
 (grb_smaa_edge_detection_to_peers), and whole sharded frames against the unsharded frame with both exchange paths
 of the C++ graph (peer-memory stores, NCCL all-gather)."""
-import os
-import signal
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -13,7 +8,6 @@ from tests import common
 from tests.test_oracle_ref_smaa import smaa_test_image
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SENTINEL = 0xA5
 
 
@@ -61,28 +55,12 @@ def test_edge_kernel_routes_rows_to_peer_windows(cuda):
     assert not counters[0].item() and not counters[1].item()  # the last CTA resets the scratch counter
 
 
-def _gpu_count():
-    import torch
-
-    return torch.cuda.device_count() if torch.cuda.is_available() else 0
-
-
 @pytest.mark.parametrize("exchange", ["peer", "nccl"])
 def test_sharded_smaa_frame_is_bit_identical(cuda, exchange):
     """4 ranks (sharing GPUs where there are fewer), equal and narrow bands, presets Low and Ultra, 4 frames each."""
     world = 4
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(common.free_port()), os.path.join(ROOT, "tests", "multi_gpu_smaa_worker.py"), "1280", "768", "300"]
-    env = dict(os.environ, GRB_SHARD_EXCHANGE=exchange)
-    proc = subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True, cwd=ROOT, env=env, start_new_session=True)
-    try:
-        out, err = proc.communicate(timeout=900)
-    except subprocess.TimeoutExpired:
-        os.killpg(proc.pid, signal.SIGKILL)  # the launcher and every rank
-        out, err = proc.communicate()
-        pytest.fail("the sharded run did not finish in 900 s:\n" + out[-3000:] + err[-3000:])
-    sys.stdout.write(out[-4000:])
-    assert proc.returncode == 0, out[-3000:] + err[-3000:]
+    rc, out, err = common.run_ranks("multi_gpu_smaa_worker.py", [1280, 768, 300], world, {"GRB_SHARD_EXCHANGE": exchange}, 900)
+    assert rc == 0, out[-3000:] + err[-3000:]
     assert out.count(f"sharded over {world} ranks == single GPU: True") == 2 * 2 * 4, out[-3000:]
     assert out.count("weights near every border: True") == 4, out[-3000:]
     if exchange == "peer":

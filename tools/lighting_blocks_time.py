@@ -11,7 +11,6 @@ nvidia-smi query in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -27,7 +26,7 @@ def main():
     torch.cuda.set_device(0)
     from granite_b200 import capi, harness
     from oracle import pyoracle as oracle
-    from tests import common
+    from tests import common, sharded
 
     capi.lib()
     capi.init()
@@ -49,9 +48,8 @@ def main():
         b.record()
         b.synchronize()
         ms.append(a.elapsed_time(b) / args.iters)
-    q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
     print(json.dumps({"kernel": "grb_deferred_lighting_blocks", "size": "3840x2160", "lights": prep.n, "ms_per_launch": ms,
-                      "card": q.stdout.strip() or "unknown"}))
+                      "card": sharded.card(0)}))
 
 
 if __name__ == "__main__":

@@ -12,14 +12,13 @@ of one measure call and of one move plus the frame that follows it, against one 
 its first frame.  A frame after a move or a re-bake brings the host G-buffer; the others find it resident.
 
 One rank per GPU: timings from ranks that share a GPU are not scaling numbers; --shared-ok runs anyway (for a check of
-the tool itself) and marks the result "one_rank_per_gpu": false.  The card's name and power limit come from a read-only
+the tool itself; tests/sharded.py's init_ranks says how ranks share a GPU) and marks the result "one_rank_per_gpu": false.  The card's name and power limit come from a read-only
 nvidia-smi query in the same run.
 """
 import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 import time
 
@@ -29,12 +28,10 @@ import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
+from granite_b200 import synth, viewer  # noqa: E402
+from tests import sharded  # noqa: E402
+
 EVERY = 16  # frames between two measure + move steps of the live schedule
-
-
-def card(index):
-    q = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    return q.stdout.strip() or "unknown"
 
 
 def main():
@@ -45,25 +42,9 @@ def main():
     ap.add_argument("--lights", type=int, default=4096)
     ap.add_argument("--shared-ok", action="store_true", help="allow more ranks than GPUs (not a scaling number)")
     args = ap.parse_args()
-    rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
-    gpus = torch.cuda.device_count()
-    if world > gpus:
-        if not args.shared_ok:
-            raise SystemExit(f"{world} ranks on {gpus} GPUs: one rank per GPU is needed for a scaling number (--shared-ok to run anyway)")
-        # ranks share a device: each names a host of its own so that NCCL accepts them (see tests/multi_gpu_worker.py)
-        os.environ["NCCL_HOSTID"] = f"granite-live-bands-rank-{rank}"
-        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
-        os.environ.setdefault("NCCL_IB_DISABLE", "1")
-    local = local % gpus
-    torch.cuda.set_device(local)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    from granite_b200 import synth, viewer
-
+    rank, world, local = sharded.init_ranks(allow_shared=args.shared_ok, refusal_hint=" (--shared-ok to run anyway)")
     w, h, frames = args.width, args.height, args.frames
-    scene = synth.make_scene(w, h)
-    lights = synth.make_lights(args.lights, aspect=w / h)
-    keep = [np.ascontiguousarray(a) for a in (scene.albedo, scene.normal, scene.pbr, scene.depth, scene.emissive)]
-    gb = viewer.Viewer.host_gbuffer(*keep)
+    scene, lights, keep, gb = sharded.inputs(w, h, args.lights, spot_fraction=0.0)
     # the camera circles the origin: the light-dense rows move from frame to frame
     views = [synth.look_at_view((1.5 * math.sin(0.05 * i), 0.6 * math.cos(0.03 * i), 8.0 + 0.5 * math.sin(0.02 * i)), (0.0, 0.0, 0.0))
              for i in range(frames)]
@@ -71,18 +52,7 @@ def main():
     stream = torch.cuda.Stream()
 
     def make(bands):
-        v = viewer.Viewer(w, h, cuda_device=local, timestamps=True, stream=stream.cuda_stream)
-        v.set_directional(scene.dir_color, scene.dir_direction)
-        v.set_lights(lights)
-        uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
-        if rank == 0:
-            uid.copy_(torch.frombuffer(bytearray(viewer.nccl_unique_id()), dtype=torch.uint8))
-        dist.broadcast(uid, 0)
-        v.init_collectives(uid.cpu().numpy().tobytes(), rank, world)
-        v.set_row_shards(bands, rank)
-        v.set_camera(scene.projection, views[0])
-        v.bake()
-        return v
+        return sharded.make_viewer(w, h, scene, lights, views[0], bands, timestamps=True, stream=stream.cuda_stream)
 
     def measured_bands(v):
         return [tuple(int(y) for y in b) for b in viewer.band_partition_measured(h, w, world, v.measure_row_cost(), align=8)]
@@ -120,9 +90,7 @@ def main():
         torch.cuda.synchronize()
         ms = a0.elapsed_time(a1)
         lighting = v.collect_timings().get("lighting", (0.0, 0))
-        v.sync()
-        dist.barrier()
-        v.close()
+        sharded.close_sharded(v)
         mine = {"rank": rank, "band": bands[rank], "lighting_ms": round(lighting[0] / max(lighting[1], 1), 4), "loop_ms": round(ms, 2),
                 "measure_host_ms": round(1e3 * float(np.median(measure_s)), 3) if measure_s else None,
                 "move_and_frame_host_ms": round(1e3 * float(np.median(move_s)), 3) if move_s else None}
@@ -146,14 +114,13 @@ def main():
         v.render_frame(gb)
         v.sync()
         s = time.perf_counter() - t0
-        dist.barrier()
-        v.close()
+        sharded.close_sharded(v)
         every = [None] * world
         dist.all_gather_object(every, round(1e3 * s, 3))
         return every
 
     result = {"workload": f"{w}x{h}, {args.lights} lights, bloom + tonemap, camera moving every frame", "ranks": world, "frames": frames,
-              "one_rank_per_gpu": world <= gpus, "gpu": card(local), "schedules": []}
+              "one_rank_per_gpu": world <= torch.cuda.device_count(), "gpu": sharded.card(local), "schedules": []}
     for schedule in ("equal, fixed", "measured once", "measure + move every 16"):
         result["schedules"].append(run(schedule))
     result["rebake_and_frame_host_ms"] = rebake()
