@@ -39,6 +39,10 @@ class GrbRows(C.Structure):
     _fields_ = [("y0", C.c_int32), ("y1", C.c_int32)]
 
 
+class GrbStripes(C.Structure):
+    _fields_ = [("first", C.c_int32), ("rows", C.c_int32), ("period", C.c_int32)]
+
+
 class GrbBloomTailOptions(C.Structure):
     _fields_ = [("u0", C.c_void_p), ("u0_rows", GrbRows), ("peer_flags", C.c_void_p), ("peer_count", C.c_int32), ("peer_epoch", C.c_uint32),
                 ("max_ctas", C.c_int32)]
@@ -96,7 +100,7 @@ ENTRY_POINTS = [
     "grb_bloom_threshold", "grb_bloom_threshold_downsample", "grb_bloom_threshold_downsample_to_peers", "grb_bloom_downsample", "grb_bloom_downsample_to_peers", "grb_peer_wait", "grb_bloom_upsample", "grb_bloom_upsample_exact",
     "grb_luminance", "grb_luminance_grid", "grb_luminance_finalize", "grb_bloom_tail", "grb_bloom_tail_ex", "grb_tonemap",
     "grb_pq10_encode", "grb_smaa_edge_detection", "grb_smaa_edge_detection_to_peers", "grb_smaa_blend_weights", "grb_smaa_neighborhood_blend", "grb_fsr_easu_constants", "grb_fsr_upscale", "grb_fsr_sharpen", "grb_fxaa", "grb_taa_resolve", "grb_taa_resolve_to_peers",
-    "grb_present_rows_to_peer",
+    "grb_present_rows_to_peer", "grb_deferred_lighting_stripes", "grb_hdr_rows_to_peers",
 ]
 
 _lib = None
@@ -153,6 +157,9 @@ def lib() -> C.CDLL:
             "grb_taa_resolve": [IMG, IMG, IMG, IMG, P, I, IMG, IMG, GrbRows, P],
             "grb_taa_resolve_to_peers": [IMG, IMG, IMG, IMG, P, I, IMG, IMG, P, P, I, I, C.c_uint32, P, GrbRows, GrbRows, P],
             "grb_present_rows_to_peer": [IMG, P, P, I, I, C.c_uint32, P, GrbRows, P],
+            "grb_deferred_lighting_stripes": [C.POINTER(GrbGBuffer), C.POINTER(GrbCamera), C.POINTER(GrbClusterParameters),
+                                              C.POINTER(GrbClusterBuffers), C.POINTER(GrbLightShadows), IMG, GrbStripes, P, P],
+            "grb_hdr_rows_to_peers": [IMG, P, P, C.POINTER(GrbRows), I, I, C.c_uint32, P, GrbStripes, P],
         }
         for name, args in sig.items():
             fn = getattr(_lib, name)

@@ -781,7 +781,26 @@ __device__ __forceinline__ void light_terms(const SurfaceP &s, const float4 l0, 
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_kernel(const LightingParams p, const PersistentArgs a)
+// Where the persistent kernel's 4-row work items (strips) lie.  Strip i of a band: rows from p.y0 + 4 i.
+struct BandStrips
+{
+	__device__ __forceinline__ int first_row(const LightingParams &p, int strip) const { return p.y0 + strip * 4; }
+};
+// Strip i of a stripe set (grb_deferred_lighting_stripes): stripe k = i / strips_per_stripe starts at first + k period,
+// and the strip lies (i mod strips_per_stripe) * 4 rows into it.  Only the last stripe can be cut by the image (p.y1).
+struct StripeSetStrips
+{
+	int first, strips_per_stripe, period;
+	__device__ __forceinline__ int first_row(const LightingParams &, int strip) const
+	{
+		const int k = strip / strips_per_stripe;
+		return first + k * period + (strip - k * strips_per_stripe) * 4;
+	}
+};
+
+// Strips: BandStrips (the rows p.y0 .. p.y1) or StripeSetStrips (grb_deferred_lighting_stripes).
+template <class Strips>
+__global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_kernel(const LightingParams p, const PersistentArgs a, const Strips strips)
 {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	// layout: [records (n_lights + 1) x 48 B][srgb LUT 1 KiB][lists kPWarps x (kListCap + 2) u16][G-buffer prefetch slots][mbarrier]
@@ -897,7 +916,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 		{
 			const unsigned r = i / n64, bx = i - r * n64;
 			it.px0 = (int)bx * 64;
-			it.py0 = p.y0 + it.strip * 4 + (int)r;
+			it.py0 = strips.first_row(p, it.strip) + (int)r;
 			it.pw = 64;
 			it.ph = 1;
 			it.x = it.px0 + 2 * lane;
@@ -906,7 +925,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 		else
 		{
 			it.px0 = i < blocks16 ? (int)i * 16 : p.hdr.w; // surplus items lie outside the image
-			it.py0 = p.y0 + it.strip * 4;
+			it.py0 = strips.first_row(p, it.strip);
 			it.pw = 16;
 			it.ph = 4;
 			it.x = it.px0 + 2 * (lane & 7);
@@ -1201,7 +1220,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 #ifdef GRB_LIGHTING_DEBUG
 		if (lane == 0)
 		{
-			const int bi = cur_by * a.blocks_x + (cur.ph == 4 ? (cur.px0 >> 4) : ((cur.py0 - p.y0 - cur_by * 4) * (a.blocks_x / 4) + (cur.px0 >> 6)));
+			const int bi = cur_by * a.blocks_x + (cur.ph == 4 ? (cur.px0 >> 4) : ((cur.py0 - strips.first_row(p, cur_by)) * (a.blocks_x / 4) + (cur.px0 >> 6)));
 			if (bi < kDbgBlocks)
 				g_dbg_block[bi] = make_uint2((uint32_t)(clock64() - t_begin), (uint32_t)(globaltimer_ns() - s_t0));
 		}
@@ -1412,7 +1431,8 @@ extern "C" int32_t grb_deferred_lighting(const GrbGBuffer *g, const GrbCamera *c
 }
 
 static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params, const GrbClusterBuffers *buf,
-                                        const GrbImage *hdr, GrbRows rows, void *schedule, void *stream, bool blocks_only, const GrbLightShadows *shadows = nullptr);
+                                        const GrbImage *hdr, GrbRows rows, void *schedule, void *stream, bool blocks_only, const GrbLightShadows *shadows = nullptr,
+                                        const GrbStripes *stripes = nullptr);
 
 extern "C" int32_t grb_deferred_lighting_scheduled(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params,
                                                    const GrbClusterBuffers *buf, const GrbImage *hdr, GrbRows rows, void *schedule, void *stream)
@@ -1451,8 +1471,28 @@ extern "C" int32_t grb_deferred_lighting_shadowed(const GrbGBuffer *g, const Grb
 	return launch_deferred_lighting(g, cam, params, buf, hdr, rows, nullptr, stream, true, shadows);
 }
 
+// Lighting of a stripe set (rows [first + k period, first + k period + rows), clipped to the image): the persistent
+// kernel takes the set's strips as its work items in one launch; the other forms run one launch per stripe.
+extern "C" int32_t grb_deferred_lighting_stripes(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params,
+                                                 const GrbClusterBuffers *buf, const GrbLightShadows *shadows, const GrbImage *hdr, GrbStripes stripes,
+                                                 void *schedule, void *stream)
+{
+	if (stripes.first < 0 || stripes.rows < 4 || stripes.rows % 4 != 0 || stripes.period < stripes.rows)
+	{
+		set_last_error("grb_deferred_lighting_stripes: stripes need first >= 0, rows a positive multiple of 4 and period >= rows");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (shadows && params && params->num_lights > 0 && (!shadows->transforms || !shadows->maps || shadows->resolution <= 0 || shadows->resolution > 16384))
+	{
+		set_last_error("grb_deferred_lighting_stripes: transforms / maps must be device arrays of num_lights entries, resolution in 1..16384");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return launch_deferred_lighting(g, cam, params, buf, hdr, GrbRows{ 0, 0 }, shadows ? nullptr : schedule, stream, shadows != nullptr, shadows, &stripes);
+}
+
 static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params, const GrbClusterBuffers *buf,
-                                        const GrbImage *hdr, GrbRows rows, void *schedule, void *stream, bool blocks_only, const GrbLightShadows *shadows)
+                                        const GrbImage *hdr, GrbRows rows, void *schedule, void *stream, bool blocks_only, const GrbLightShadows *shadows,
+                                        const GrbStripes *stripes)
 {
 	if (!g || !cam || !params || !buf || !hdr)
 	{
@@ -1490,7 +1530,7 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		set_last_error("grb_deferred_lighting: lights must be 16-byte aligned");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	rows = full_rows(rows, h);
+	rows = stripes ? GrbRows{ stripes->first, h } : full_rows(rows, h);
 	if (rows.y1 <= rows.y0)
 		return GRB_OK;
 
@@ -1570,7 +1610,9 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 				if (err == cudaSuccess)
 					err = cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
 				if (err == cudaSuccess)
-					err = cudaFuncSetAttribute(deferred_lighting_persistent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+					err = cudaFuncSetAttribute(deferred_lighting_persistent_kernel<BandStrips>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+				if (err == cudaSuccess)
+					err = cudaFuncSetAttribute(deferred_lighting_persistent_kernel<StripeSetStrips>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
 				void *q = nullptr;
 				if (err == cudaSuccess)
 					err = cudaGetSymbolAddress(&q, g_light_queue);
@@ -1588,6 +1630,15 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		PersistentArgs a;
 		a.blocks_x = 4 * ((w + 63) / 64); // items per strip: 4 rows of 64x1 blocks, or ceil(w / 16) 16x4 blocks (+ empty ones)
 		a.blocks_y = (rows.y1 - rows.y0 + 3) / 4;
+		StripeSetStrips strips = {};
+		if (stripes)
+		{
+			// every stripe but the last that starts inside the image is whole
+			const int spp = stripes->rows / 4, count = (h - stripes->first + stripes->period - 1) / stripes->period;
+			const int last_rows = std::min(stripes->rows, h - (stripes->first + (count - 1) * stripes->period));
+			strips = StripeSetStrips{ stripes->first, spp, stripes->period };
+			a.blocks_y = (count - 1) * spp + (last_rows + 3) / 4;
+		}
 		a.total_items = a.blocks_x * a.blocks_y;
 		a.schedule = static_cast<uint32_t *>(schedule);
 		a.n_lights = params->num_lights;
@@ -1603,25 +1654,37 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		if (smem <= (size_t)di.smem_max)
 		{
 			const int ctas = std::min(di.sm_count, std::max(1, (a.blocks_x * a.blocks_y + kPWarps - 1) / kPWarps));
-			deferred_lighting_persistent_kernel<<<ctas, 32 * kPWarps, smem, as_stream(stream)>>>(p, a);
+			if (stripes)
+				deferred_lighting_persistent_kernel<<<ctas, 32 * kPWarps, smem, as_stream(stream)>>>(p, a, strips);
+			else
+				deferred_lighting_persistent_kernel<<<ctas, 32 * kPWarps, smem, as_stream(stream)>>>(p, a, BandStrips{});
 			return check_launch("grb_deferred_lighting");
 		}
 	}
-	if (pairs)
-	{
-		dim3 grid2((w / 2 + 8 * kWarpsPerCta - 1) / (8 * kWarpsPerCta), (rows.y1 - rows.y0 + 3) / 4, 1);
-		deferred_lighting2_kernel<<<grid2, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
-		return check_launch("grb_deferred_lighting");
-	}
-	dim3 grid((w + 8 * kWarpsPerCta - 1) / (8 * kWarpsPerCta), (rows.y1 - rows.y0 + 3) / 4, 1);
-	if (hdr16 && shadows)
-		deferred_lighting_kernel<true, true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
-	else if (hdr16)
-		deferred_lighting_kernel<false, true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
-	else if (shadows)
-		deferred_lighting_kernel<true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
-	else
-		deferred_lighting_kernel<false><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+	auto launch_rows = [&](int y0, int y1) {
+		p.y0 = y0;
+		p.y1 = y1;
+		if (pairs)
+		{
+			dim3 grid2((w / 2 + 8 * kWarpsPerCta - 1) / (8 * kWarpsPerCta), (y1 - y0 + 3) / 4, 1);
+			deferred_lighting2_kernel<<<grid2, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+			return;
+		}
+		dim3 grid((w + 8 * kWarpsPerCta - 1) / (8 * kWarpsPerCta), (y1 - y0 + 3) / 4, 1);
+		if (hdr16 && shadows)
+			deferred_lighting_kernel<true, true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+		else if (hdr16)
+			deferred_lighting_kernel<false, true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+		else if (shadows)
+			deferred_lighting_kernel<true><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+		else
+			deferred_lighting_kernel<false><<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p);
+	};
+	if (!stripes)
+		launch_rows(rows.y0, rows.y1);
+	else // the forms the persistent kernel does not serve: one launch per stripe
+		for (int y = stripes->first; y < h; y += stripes->period)
+			launch_rows(y, std::min(y + stripes->rows, h));
 	return check_launch("grb_deferred_lighting");
 }
 

@@ -173,6 +173,40 @@ __global__ void __launch_bounds__(256) present_rows_kernel(const uint8_t *__rest
 	peer_publish(targets);
 }
 
+// Lighting in stripes on a row-sharded frame: each rank stores the rows it lit that another rank's lighting rows hold
+// into that rank's HDR slot (IPC-mapped peer memory), then publishes in every rank's flag array (grb_peer.cuh).
+// blockIdx.y walks the rows of the stripe set; one thread moves 16 bytes (a 16-byte load and store when the row pitch
+// and every base allow it, 4-byte words otherwise and for a row's last bytes).  Texels are 4 or 8 bytes, so a row is a
+// whole number of words.
+struct PeerRowsArg
+{
+	GrbRows rows[GRB_MAX_PEERS]; // [rank] that rank's lighting rows: the rows its slot takes
+};
+
+template <bool Vec16>
+__global__ void __launch_bounds__(256) hdr_rows_to_peers_kernel(const uint8_t *__restrict__ src, int pitch, int row_bytes, GrbStripes stripes,
+                                                              int self, PeerRowsArg peer_rows, PeerTargets targets)
+{
+	__builtin_assume(threadIdx.y == 0); // 1-D blocks: peer_publish's leader test is threadIdx.x == 0
+	const int x = 16 * (int)(blockIdx.x * blockDim.x + threadIdx.x);
+	const int i = (int)blockIdx.y, k = i / stripes.rows;
+	const int y = stripes.first + k * stripes.period + (i - k * stripes.rows);
+	if (x < row_bytes)
+		for (int q = 0; q < targets.count; q++)
+		{
+			if (q == self || y < peer_rows.rows[q].y0 || y >= peer_rows.rows[q].y1)
+				continue;
+			const size_t at = (size_t)y * pitch + (size_t)x;
+			uint8_t *dst = static_cast<uint8_t *>(targets.data[q]);
+			if (Vec16 && x + 16 <= row_bytes)
+				*reinterpret_cast<uint4 *>(dst + at) = __ldg(reinterpret_cast<const uint4 *>(src + at));
+			else
+				for (int j = 0; j < 16 && x + j < row_bytes; j += 4)
+					*reinterpret_cast<uint32_t *>(dst + at + j) = __ldg(reinterpret_cast<const uint32_t *>(src + at + j));
+		}
+	peer_publish(targets);
+}
+
 // ------------------------------------------------------------------------------- K10
 // Average log-luminance.  The reference sums with one 8x8 workgroup: each invocation adds its
 // strided samples in (y-iter, x-iter) order, then a shared-memory tree 32,16,8,4,2 and a final
@@ -1062,6 +1096,69 @@ extern "C" int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint
 	else
 		present_rows_kernel<false><<<grid, block, 0, as_stream(stream)>>>(s, d, src->row_pitch, src->width, own.y0, targets);
 	return check_launch("grb_present_rows_to_peer");
+}
+
+extern "C" int32_t grb_hdr_rows_to_peers(const GrbImage *hdr, void *const *peer_images, uint32_t *const *peer_flags, const GrbRows *peer_rows,
+                                         int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, GrbStripes stripes,
+                                         void *stream)
+{
+	if (!hdr || !hdr->data || !peer_rows)
+	{
+		set_last_error("grb_hdr_rows_to_peers: null pointer");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	PeerTargets targets;
+	if (!peer_targets_from("grb_hdr_rows_to_peers", peer_images, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
+		return GRB_ERR_INVALID_ARGUMENT;
+	const int texel = texel_bytes(hdr->format);
+	if ((texel != 4 && texel != 8) || hdr->width <= 0 || hdr->height <= 0 || hdr->row_pitch < hdr->width * texel || (hdr->row_pitch % 4) != 0)
+	{
+		set_last_error("grb_hdr_rows_to_peers: hdr must be an image of 4- or 8-byte texels (B10G11R11_UFLOAT or R16G16B16A16_SFLOAT)");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (hdr->height > 65535)
+	{
+		set_last_error("grb_hdr_rows_to_peers: hdr may have at most 65535 rows (one grid row per image row)");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (stripes.first < 0 || stripes.rows < 1 || stripes.period < stripes.rows)
+	{
+		set_last_error("grb_hdr_rows_to_peers: stripes need first >= 0, rows >= 1 and period >= rows");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	PeerRowsArg rows_arg = {};
+	bool vec16 = (hdr->row_pitch % 16) == 0 && (reinterpret_cast<uintptr_t>(hdr->data) % 16) == 0;
+	for (int q = 0; q < peer_count; q++)
+	{
+		const GrbRows r = peer_rows[q];
+		if (r.y0 < 0 || r.y1 < r.y0 || r.y1 > hdr->height)
+		{
+			set_last_error("grb_hdr_rows_to_peers: peer_rows[q] must be a range inside the image (empty allowed)");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+		if (q != flag_index && peer_images[q] == hdr->data)
+		{
+			set_last_error("grb_hdr_rows_to_peers: a peer's slot must be distinct from hdr");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+		rows_arg.rows[q] = r;
+		vec16 = vec16 && (reinterpret_cast<uintptr_t>(peer_images[q]) % 16) == 0;
+	}
+	// rows of the stripe set inside the image: whole stripes, then the part of the last one above the image's end
+	int row_count = 0;
+	if (stripes.first < hdr->height)
+	{
+		const int count = (hdr->height - stripes.first + stripes.period - 1) / stripes.period;
+		row_count = (count - 1) * stripes.rows + std::min(stripes.rows, hdr->height - (stripes.first + (count - 1) * stripes.period));
+	}
+	const int row_bytes = hdr->width * texel;
+	const dim3 block(256), grid = peer_grid(row_count, dim3((unsigned)((row_bytes + 16 * 256 - 1) / (16 * 256)), (unsigned)row_count));
+	const auto *s = static_cast<const uint8_t *>(hdr->data);
+	if (vec16)
+		hdr_rows_to_peers_kernel<true><<<grid, block, 0, as_stream(stream)>>>(s, hdr->row_pitch, row_count > 0 ? row_bytes : 0, stripes, flag_index, rows_arg, targets);
+	else
+		hdr_rows_to_peers_kernel<false><<<grid, block, 0, as_stream(stream)>>>(s, hdr->row_pitch, row_count > 0 ? row_bytes : 0, stripes, flag_index, rows_arg, targets);
+	return check_launch("grb_hdr_rows_to_peers");
 }
 
 static int32_t bloom_upsample_impl(const GrbImage *in, const GrbImage *out, GrbRows rows, void *stream, bool allow_tiles)

@@ -152,6 +152,36 @@ def deferred_lighting_shadowed(gb: GBufferDevice, cam: capi.GrbCamera, cluster: 
                                                          C.byref(sh), C.byref(img), capi.rows(rows), capi.stream_ptr()), "grb_deferred_lighting_shadowed")
 
 
+def deferred_lighting_stripes(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDevice, hdr: torch.Tensor, stripes, schedule=None, shadows=None):
+    """grb_deferred_lighting_stripes over the stripe set stripes = (first, rows, period).  shadows: None, or
+    (transforms, map_table, resolution) as for deferred_lighting_shadowed."""
+    img = _hdr_img(hdr)
+    sh = None
+    if shadows is not None:
+        transforms, map_table, resolution = shadows
+        sh = C.byref(capi.GrbLightShadows(_ptr(transforms), _ptr(map_table), int(resolution), 0))
+    capi.check(capi.lib().grb_deferred_lighting_stripes(C.byref(gb.struct), C.byref(cam), C.byref(cluster.params), C.byref(cluster.buffers), sh,
+                                                        C.byref(img), capi.GrbStripes(*stripes), None if schedule is None else _ptr(schedule),
+                                                        capi.stream_ptr()),
+               "grb_deferred_lighting_stripes")
+
+
+def hdr_rows_to_peers(hdr_t, slots, flag_arrays, peer_rows, flag_index, epoch, counter_t, stripes, width=None):
+    """grb_hdr_rows_to_peers with every rank's HDR slot and flag array as tensors on this device: hdr_t and slots[q]
+    (H, P) int32 (B10G11R11) or (H, P, 4) int16 (RGBA16F), the image the first `width` texels of each row (all P by
+    default); peer_rows[q] = rank q's lighting rows (y0, y1)."""
+    img = _hdr_img(hdr_t)
+    if width is not None:
+        img.width = int(width)
+    n = len(slots)
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    rows = (capi.GrbRows * n)(*[capi.GrbRows(int(a), int(b)) for a, b in peer_rows])
+    capi.check(capi.lib().grb_hdr_rows_to_peers(C.byref(img), images, flags, rows, n, int(flag_index), int(epoch), _ptr(counter_t),
+                                                capi.GrbStripes(*stripes), capi.stream_ptr()),
+               "grb_hdr_rows_to_peers")
+
+
 def _img16(t):
     return capi.image(t, capi.FORMAT_R16G16B16A16_SFLOAT)
 

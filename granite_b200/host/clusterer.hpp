@@ -45,6 +45,9 @@ public:
 		lit_y1 = y1;
 		lit_height = height;
 	}
+	// Row-sharded frames lit in stripes: the tile-row ranges under this rank's stripes (StripePlan::tile_rows), binned
+	// one range at a time; they replace the lit pixel rows above.  Empty: off (default).
+	void set_lit_tile_ranges(std::vector<GrbRows> ranges) { lit_tile_ranges = std::move(ranges); }
 	// Shadowed positional lights (clusterer.cpp:78-81,173-176): the lighting pass multiplies each light by the PCF
 	// comparison sample of its shadow map (PositionalLight::set_shadow_map).  RENDERING the maps is the caller's
 	// (clusterer.cpp:206-330 is rasterisation, outside the path); the clusterer computes the per-light shadow
@@ -119,6 +122,7 @@ private:
 	bool enable_clustering = true;
 	bool async_compute = false;
 	int lit_y0 = 0, lit_y1 = 0, lit_height = 0;
+	std::vector<GrbRows> lit_tile_ranges;
 
 	GrbClusterParameters parameters = {};
 	std::vector<PositionalFragmentInfo> lights;

@@ -151,20 +151,29 @@ bool NcclCollectives::init(const unsigned char id_bytes[NcclUniqueIdBytes], unsi
 
 bool NcclCollectives::all_gather_rows(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<GrbRows> &rows)
 {
+	std::vector<std::vector<GrbRows>> lists;
+	for (const GrbRows &r : rows)
+		lists.push_back({ r });
+	return all_gather_row_lists(cmd, image, lists);
+}
+
+bool NcclCollectives::all_gather_row_lists(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<std::vector<GrbRows>> &rows)
+{
 	if (!comm || rows.size() != world)
 		return false;
-	// Bands differ in height, so this is a grouped set of broadcasts (one root per band), which
+	// Bands differ in height, so this is a grouped set of broadcasts (one root per range), which
 	// NCCL fuses into a single launch over NVLink.
 	auto &a = api();
 	auto *base = static_cast<unsigned char *>(image.get_image().get_device_pointer());
 	const size_t pitch = image.get_image().get_row_pitch();
 	bool ok = nccl_ok(a.GroupStart(), "ncclGroupStart");
 	for (unsigned r = 0; r < world && ok; r++)
-	{
-		size_t bytes = (size_t)(rows[r].y1 - rows[r].y0) * pitch;
-		void *p = base + (size_t)rows[r].y0 * pitch;
-		ok = nccl_ok(a.Broadcast(p, p, bytes, ncclInt8, (int)r, comm, cmd.get_stream_handle()), "ncclBroadcast");
-	}
+		for (const GrbRows &range : rows[r])
+		{
+			size_t bytes = (size_t)(range.y1 - range.y0) * pitch;
+			void *p = base + (size_t)range.y0 * pitch;
+			ok = ok && nccl_ok(a.Broadcast(p, p, bytes, ncclInt8, (int)r, comm, cmd.get_stream_handle()), "ncclBroadcast");
+		}
 	ok = nccl_ok(a.GroupEnd(), "ncclGroupEnd") && ok;
 	return ok ? true : collective_failed("all_gather_rows");
 }

@@ -24,6 +24,7 @@ public:
 	unsigned get_rank() const override { return rank; }
 	unsigned get_world_size() const override { return world; }
 	bool all_gather_rows(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<GrbRows> &rows) override;
+	bool all_gather_row_lists(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<std::vector<GrbRows>> &rows) override;
 	bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) override;
 	bool all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, size_t count) override;
 	// Peer-memory exchange: two image slots + a flag array per rank, cudaIpc-mapped into every
@@ -46,7 +47,7 @@ private:
 		std::vector<void *> opened;
 		uint32_t epoch = 0;
 	};
-	PeerState channels[(size_t)PeerChannel::Present + 1]; // [PeerChannel]
+	PeerState channels[(size_t)PeerChannel::HdrStripes + 1]; // [PeerChannel]
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);
 };

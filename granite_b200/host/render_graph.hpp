@@ -48,6 +48,14 @@ public:
 	virtual unsigned get_world_size() const = 0;
 	// Every rank contributes rows [rows[r].y0, rows[r].y1) of an image all ranks hold at full size.
 	virtual bool all_gather_rows(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<GrbRows> &rows) = 0;
+	// The same with a list of row ranges per rank (the stripes of a frame lit in stripes); false = not available.
+	virtual bool all_gather_row_lists(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<std::vector<GrbRows>> &rows)
+	{
+		(void)cmd;
+		(void)image;
+		(void)rows;
+		return false;
+	}
 	virtual bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) = 0;
 	// Exact integer sum over ranks (modulo 2^32), in place on `stream`; false = not available.  For small host-driven
 	// reductions outside the graph (the viewer's sharded row-cost measurement).
@@ -74,6 +82,8 @@ public:
 		            // filled (host/post/temporal.cpp)
 		Present,    // the bands of the final image, pushed into the presenting rank's slots only (the "present" pass of
 		            // scene_viewer.cpp)
+		HdrStripes, // the HDR-main rows a rank lit in stripes that other ranks' lighting rows hold (the "lighting" and
+		            // "lighting-exchange" passes of scene_viewer.cpp)
 	};
 	struct PeerSlot
 	{

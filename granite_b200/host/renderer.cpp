@@ -6,7 +6,7 @@
 namespace Granite
 {
 void DeferredLightRenderer::render_light(Vulkan::CommandBuffer &cmd, const RenderContext &context, const GBufferViews &gb, Vulkan::ImageView &hdr,
-                                         GrbRows rows, void *schedule, bool blocks_form)
+                                         GrbRows rows, void *schedule, bool blocks_form, const GrbStripes *stripes)
 {
 	auto *light = context.get_lighting_parameters();
 	if (!light || !gb.albedo || !gb.normal || !gb.pbr || !gb.depth)
@@ -59,7 +59,11 @@ void DeferredLightRenderer::render_light(Vulkan::CommandBuffer &cmd, const Rende
 	// post chain of the previous frame can interleave with this pass (see grb_deferred_lighting_blocks).
 	// POSITIONAL_LIGHTS_SHADOW (renderer.cpp:1124-1131): the clusterer holds the shadow transforms and map pointers
 	const GrbLightShadows shadows = light->cluster->get_light_shadows();
-	if (shadows.maps)
+	if (stripes)
+		cmd.check(grb_deferred_lighting_stripes(&g, &cam, &params, &buffers, shadows.maps ? &shadows : nullptr, &hdr_img, *stripes, schedule,
+		                                        cmd.get_stream_handle()),
+		          "grb_deferred_lighting_stripes");
+	else if (shadows.maps)
 		cmd.check(grb_deferred_lighting_shadowed(&g, &cam, &params, &buffers, &shadows, &hdr_img, rows, cmd.get_stream_handle()), "grb_deferred_lighting_shadowed");
 	else if (blocks_form)
 		cmd.check(grb_deferred_lighting_blocks(&g, &cam, &params, &buffers, &hdr_img, rows, cmd.get_stream_handle()), "grb_deferred_lighting_blocks");
@@ -104,6 +108,12 @@ void DeferredLightingPass::build_render_pass(Vulkan::CommandBuffer &cmd)
 	// persistent CTA per SM), as before the frame was phased.
 	static const bool sharded_blocks = getenv("GRB_SHARDED_BLOCKS") != nullptr;
 	const bool sharded = graph->is_sharded() && graph->get_shard_count() > 1;
+	if (push)
+	{
+		DeferredLightRenderer::render_light(cmd, context, gb, hdr, GrbRows{ 0, 0 }, schedule, false, &stripes);
+		push(cmd, hdr);
+		return;
+	}
 	DeferredLightRenderer::render_light(cmd, context, gb, hdr, graph->is_sharded() ? graph->get_shard_plan().lighting : GrbRows{ 0, 0 }, schedule,
 	                                    sharded && sharded_blocks);
 }

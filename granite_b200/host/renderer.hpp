@@ -28,8 +28,10 @@ public:
 	// schedule: optional device buffer of grb_lighting_schedule_bytes(height) bytes kept across frames.
 	// blocks_form: the non-persistent kernel (grb_deferred_lighting_blocks) -- what a row-sharded frame uses
 	// on every rank, so that the post chain waiting for a peer's band can interleave with this pass.
+	// stripes: light that stripe set instead of `rows` (grb_deferred_lighting_stripes; row-sharded frames lit in stripes).
 	static void render_light(Vulkan::CommandBuffer &cmd, const RenderContext &context, const GBufferViews &gbuffer,
-	                         Vulkan::ImageView &hdr, GrbRows rows, void *schedule = nullptr, bool blocks_form = false);
+	                         Vulkan::ImageView &hdr, GrbRows rows, void *schedule = nullptr, bool blocks_form = false,
+	                         const GrbStripes *stripes = nullptr);
 };
 
 // The "lighting" pass: reads albedo/normal/pbr/depth attachments + the cluster buffers, writes
@@ -56,5 +58,16 @@ public:
 	// extra rows around a row shard that downstream passes (bloom threshold, FXAA) read
 	void set_shard_halo(unsigned rows) { halo_rows = rows; }
 	void set_schedule(RenderBufferResource &schedule) { res_schedule = &schedule; }
+	// Row-sharded frames lit in stripes: the pass lights `stripes` instead of its lighting rows, then calls `push` on
+	// the same stream with HDR-main (the rows the other ranks read go to them: scene_viewer.cpp).
+	void set_stripes(GrbStripes stripes_, std::function<void(Vulkan::CommandBuffer &, Vulkan::ImageView &)> push_)
+	{
+		stripes = stripes_;
+		push = std::move(push_);
+	}
+
+private:
+	GrbStripes stripes = {};
+	std::function<void(Vulkan::CommandBuffer &, Vulkan::ImageView &)> push;
 };
 } // namespace Granite

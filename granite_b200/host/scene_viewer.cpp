@@ -65,6 +65,14 @@ struct GrbhViewer
 	// grbh_viewer_move_row_shards ran since the last frame: the resident G-buffer, the last output and the last depth
 	// image hold the old layout's rows until a frame (which must bring the host G-buffer) renders on the new one
 	bool bands_moved = false;
+	// row-sharded frames lit in stripes of this many rows (0: off; grbh_viewer_set_lighting_stripes), and what this
+	// frame's lighting pass left for its "lighting-exchange" pass
+	unsigned lighting_stripes = 0;
+	struct StripeExchange
+	{
+		bool peer = false;
+		RenderGraphCollectives::PeerSlot slot;
+	} stripe_exchange;
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
@@ -116,6 +124,19 @@ struct GrbhViewer
 	// rows of the render-resolution inputs this rank must hold: its band + the halo the bloom
 	// threshold (and FXAA through the tonemap, TAA's neighbourhood, FSR's window) reaches into
 	GrbRows input_rows() const { return shard_plan().lighting; }
+	bool striped() const { return lighting_stripes > 0 && bands.size() > 1; }
+	StripePlan stripe_plan() const
+	{
+		return compute_stripe_plan((unsigned)config.width, (unsigned)config.height, bands, rank, uses_fxaa(), smaa_quality(), uses_taa(), lighting_stripes,
+		                           (unsigned)config.cluster_res[1]);
+	}
+	// rank r's stripes: every bands.size()-th stripe from stripe r
+	GrbStripes stripes_of(unsigned r) const
+	{
+		return GrbStripes{ (int32_t)(r * lighting_stripes), (int32_t)lighting_stripes, (int32_t)(bands.size() * lighting_stripes) };
+	}
+	// the G-buffer rows this rank must hold
+	std::vector<GrbRows> upload_ranges() const { return striped() ? stripe_plan().upload : std::vector<GrbRows>{ input_rows() }; }
 	bool sharded_presenting() const { return bands.size() > 1 && present_rank >= 0; }
 
 	// the device-to-host copy of this rank's rows of the final image (the whole frame on the presenting rank), on the
@@ -127,12 +148,14 @@ struct GrbhViewer
 		if (!res || !host)
 			return;
 		auto &view_ = graph.get_physical_texture_resource(*res);
-		GrbRows r = input_rows();
 		size_t pitch = (size_t)render_width() * texel;
-		auto *dst = static_cast<uint8_t *>(view_.get_image().get_device_pointer()) + (size_t)r.y0 * pitch;
-		auto *src = static_cast<const uint8_t *>(host) + (size_t)r.y0 * pitch;
-		Vulkan::cuda_ok(cudaMemcpyAsync(dst, src, pitch * (size_t)(r.y1 - r.y0), cudaMemcpyHostToDevice, reinterpret_cast<cudaStream_t>(cmd.get_stream())),
-		                "G-buffer upload");
+		for (const GrbRows &r : upload_ranges())
+		{
+			auto *dst = static_cast<uint8_t *>(view_.get_image().get_device_pointer()) + (size_t)r.y0 * pitch;
+			auto *src = static_cast<const uint8_t *>(host) + (size_t)r.y0 * pitch;
+			Vulkan::cuda_ok(cudaMemcpyAsync(dst, src, pitch * (size_t)(r.y1 - r.y0), cudaMemcpyHostToDevice, reinterpret_cast<cudaStream_t>(cmd.get_stream())),
+			                "G-buffer upload");
+		}
 	}
 
 	void bake_render_graph();
@@ -171,6 +194,7 @@ void GrbhViewer::bake_render_graph()
 	}
 	else
 		cluster.set_lit_pixel_rows(0, 0, 0);
+	cluster.set_lit_tile_ranges(striped() ? stripe_plan().tile_rows : std::vector<GrbRows>{});
 	cluster.add_render_passes(graph);
 	lighting.cluster = &cluster;
 	context.set_lighting_parameters(&lighting);
@@ -240,6 +264,57 @@ void GrbhViewer::bake_render_graph()
 	lighting_pass.set_render_pass_interface(light_iface);
 
 	std::string light_output = "HDR-main";
+	if (striped())
+	{
+		// Lighting in stripes (DESIGN.md section 5, "Lighting in stripes"): the lighting pass lights this rank's stripes
+		// and pushes the rows other ranks' lighting rows hold into their slots; "lighting-exchange" waits for every
+		// rank's push and copies the rows this rank received into HDR-main.  It rewrites HDR-main in place, so every
+		// reader of the lit image (TAA, threshold, tonemap, ui / pq10) follows it through the graph's dependencies.
+		light_iface->set_stripes(stripes_of(rank), [this](Vulkan::CommandBuffer &cmd, Vulkan::ImageView &hdr) {
+			const GrbImage image = hdr.as_grb();
+			stripe_exchange.peer = graph.get_collectives()->peer_exchange_begin_frame(
+			    RenderGraphCollectives::PeerChannel::HdrStripes, (size_t)image.row_pitch * (size_t)image.height, stripe_exchange.slot);
+			if (!stripe_exchange.peer)
+				return;
+			const RenderGraphCollectives::PeerSlot &slot = stripe_exchange.slot;
+			const std::vector<GrbRows> lighting_rows = graph.get_shard_plan_rows(&ShardPlan::lighting);
+			cmd.check(grb_hdr_rows_to_peers(&image, slot.images, slot.flags, lighting_rows.data(), (int32_t)slot.count, (int32_t)rank, slot.epoch,
+			                                slot.counter, stripes_of(rank), cmd.get_stream_handle()),
+			          "grb_hdr_rows_to_peers");
+		});
+		auto &exchange = graph.add_pass("lighting-exchange", RENDER_GRAPH_QUEUE_GRAPHICS_BIT);
+		auto &lit = exchange.add_color_output("HDR-lit", hdr_info, "HDR-main");
+		exchange.set_build_render_pass([this, &lit](Vulkan::CommandBuffer &cmd) {
+			auto &view_ = graph.get_physical_texture_resource(lit);
+			if (stripe_exchange.peer)
+			{
+				const RenderGraphCollectives::PeerSlot &slot = stripe_exchange.slot;
+				auto stream = reinterpret_cast<cudaStream_t>(cmd.get_stream());
+				cmd.check(grb_peer_wait(slot.flags[rank], (int32_t)slot.count, slot.epoch, stream), "grb_peer_wait");
+				const GrbImage image = view_.as_grb();
+				const size_t pitch = (size_t)image.row_pitch;
+				auto *dst = static_cast<uint8_t *>(image.data);
+				const auto *src = static_cast<const uint8_t *>(slot.images[rank]);
+				for (const GrbRows &r : stripe_plan().receive)
+					Vulkan::cuda_ok(cudaMemcpyAsync(dst + (size_t)r.y0 * pitch, src + (size_t)r.y0 * pitch, pitch * (size_t)(r.y1 - r.y0),
+					                                cudaMemcpyDeviceToDevice, stream),
+					                "lighting-exchange copy");
+				return;
+			}
+			// without peer memory: every rank's stripes to every rank, in place
+			std::vector<std::vector<GrbRows>> lists;
+			for (unsigned r = 0; r < bands.size(); r++)
+			{
+				const GrbStripes s = stripes_of(r);
+				lists.emplace_back();
+				for (int y = s.first; y < config.height; y += s.period)
+					lists.back().push_back(GrbRows{ y, std::min(y + s.rows, config.height) });
+			}
+			if (!graph.get_collectives()->all_gather_row_lists(cmd, view_, lists))
+				throw std::runtime_error("lighting-exchange: the all-gather of the stripes failed");
+		});
+		light_output = "HDR-lit";
+	}
 
 	// ---- AA before the post chain (TAA) ----
 	PostAAType before = PostAAType::None;
@@ -453,12 +528,13 @@ int32_t GrbhViewer::measure_row_cost_sharded(uint32_t *out, int groups)
 	if (bands_moved)
 		return fail("grbh_viewer_measure_row_cost: the bands moved (grbh_viewer_move_row_shards) since the last frame; render a frame first");
 	for (const GrbRows &r : graph.get_shard_plan_rows(&ShardPlan::render_own))
-		if (r.y0 % 4 != 0)
+		if (!striped() && r.y0 % 4 != 0)
 			return fail("grbh_viewer_measure_row_cost: a row-sharded measurement needs every cut on a multiple of 4 rows (render row " +
 			            std::to_string(r.y0) + ")");
 	RenderGraphCollectives *coll = graph.get_collectives();
 	device->wait_idle();
-	const GrbRows rows = shard_plan().render_own;
+	// the rows whose depth this rank holds and whose tiles it binned: its stripes (multiples of 8 rows), or its band
+	const std::vector<GrbRows> measured = striped() ? stripe_plan().lit : std::vector<GrbRows>{ shard_plan().render_own };
 	GrbImage depth = graph.get_physical_texture_resource(*res_depth).as_grb();
 	GrbCamera cam;
 	if (grbh_viewer_get_camera(this, &cam, nullptr, nullptr) != 0)
@@ -470,7 +546,9 @@ int32_t GrbhViewer::measure_row_cost_sharded(uint32_t *out, int groups)
 	if (!Vulkan::cuda_ok(cudaMalloc(&dev, sizeof(uint32_t) * groups), "cudaMalloc"))
 		return fail("cudaMalloc failed");
 	bool ok = Vulkan::cuda_ok(cudaMemsetAsync(dev, 0, sizeof(uint32_t) * groups, stream), "cudaMemsetAsync");
-	const int32_t rc = ok ? grb_lighting_row_cost(&depth, &cam, &params, &buffers, rows, dev + rows.y0 / 4, stream) : GRB_OK;
+	int32_t rc = GRB_OK;
+	for (size_t i = 0; ok && rc == GRB_OK && i < measured.size(); i++)
+		rc = grb_lighting_row_cost(&depth, &cam, &params, &buffers, measured[i], dev + measured[i].y0 / 4, stream);
 	const std::string kernel_error = rc != GRB_OK ? grb_last_error_string() : "";
 	// every rank joins the reduction, also one whose own part failed, so that no peer waits in it alone
 	const bool reduced = coll && coll->all_reduce_sum_u32(stream, dev, (size_t)groups);
@@ -806,6 +884,19 @@ extern "C" int32_t grbh_viewer_set_present_rank(GrbhViewer *v, int32_t rank)
 	return 0;
 }
 
+extern "C" int32_t grbh_viewer_set_lighting_stripes(GrbhViewer *v, int32_t stripe_rows)
+{
+	if (!v)
+		return fail("null viewer");
+	if (stripe_rows < 0 || stripe_rows % 8 != 0)
+		return fail("grbh_viewer_set_lighting_stripes: stripe_rows must be 0 (off) or a positive multiple of 8 (got " + std::to_string(stripe_rows) + ")");
+	if (stripe_rows > 0 && v->upscales())
+		return fail("grbh_viewer_set_lighting_stripes: lighting in stripes is not supported with FSR 1 upscaling (resolution_scale < 1)");
+	v->lighting_stripes = (unsigned)stripe_rows;
+	v->baked = false;
+	return 0;
+}
+
 extern "C" int32_t grbh_viewer_move_row_shards(GrbhViewer *v, const GrbRows *bands, int32_t count)
 {
 	if (!v || !bands || count <= 0)
@@ -915,6 +1006,48 @@ extern "C" int32_t grbh_shard_plan_fsr(int32_t width, int32_t height, int32_t re
 	for (int i = 0; i < 12; i++)
 		out12[i] = all[i];
 	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_shard_plan_stripes(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t post_aa,
+                                           int32_t stripe_rows, int32_t cluster_rows, GrbRows *out, int32_t capacity, int32_t *counts)
+{
+	const bool known_aa = post_aa == GRBH_AA_NONE || post_aa == GRBH_AA_FXAA || (post_aa >= GRBH_AA_SMAA_LOW && post_aa <= GRBH_AA_SMAA_ULTRA) ||
+	                      (post_aa >= GRBH_AA_TAA_LOW && post_aa <= GRBH_AA_TAA_HIGH) || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	if (width <= 0 || height <= 0 || count < 0 || (count && !bands) || (count && (rank < 0 || rank >= count)) || (!count && rank != 0) || !known_aa ||
+	    cluster_rows <= 0 || capacity < 0 || (capacity && !out) || !counts)
+		return fail("grbh_shard_plan_stripes: bad arguments");
+	GRBH_TRY
+	std::vector<GrbRows> b(bands, bands + count);
+	const bool fxaa = post_aa == GRBH_AA_FXAA || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	const bool taa = (post_aa >= GRBH_AA_TAA_LOW && post_aa <= GRBH_AA_TAA_HIGH) || post_aa == GRBH_AA_TAA_HIGH_PLUS_FXAA;
+	const int smaa = post_aa >= GRBH_AA_SMAA_LOW && post_aa <= GRBH_AA_SMAA_ULTRA ? post_aa - GRBH_AA_SMAA_LOW : -1;
+	StripePlan sp;
+	try
+	{
+		sp = compute_stripe_plan((unsigned)width, (unsigned)height, b, (unsigned)rank, fxaa, smaa, taa, stripe_rows > 0 ? (unsigned)stripe_rows : 0u,
+		                         (unsigned)cluster_rows);
+	}
+	catch (const std::invalid_argument &e)
+	{
+		return fail(std::string("grbh_shard_plan_stripes: ") + e.what());
+	}
+	std::vector<const std::vector<GrbRows> *> lists = { &sp.lit, &sp.receive, &sp.upload, &sp.tile_rows };
+	for (const auto &p : sp.push)
+		lists.push_back(&p);
+	size_t total = 0;
+	for (const auto *l : lists)
+		total += l->size();
+	if (total > (size_t)capacity)
+		return fail("grbh_shard_plan_stripes: the plan has " + std::to_string(total) + " ranges, capacity is " + std::to_string(capacity));
+	size_t at = 0;
+	for (size_t i = 0; i < lists.size(); i++)
+	{
+		counts[i] = (int32_t)lists[i]->size();
+		for (const GrbRows &r : *lists[i])
+			out[at++] = r;
+	}
+	return (int32_t)total;
 	GRBH_CATCH
 }
 

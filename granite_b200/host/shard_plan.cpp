@@ -140,6 +140,81 @@ ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<
 	return p;
 }
 
+namespace
+{
+// The ranges of `rows` (in increasing order of y0) with overlapping or touching ones merged.
+std::vector<GrbRows> merged(std::vector<GrbRows> rows)
+{
+	std::sort(rows.begin(), rows.end(), [](const GrbRows &a, const GrbRows &b) { return a.y0 < b.y0; });
+	std::vector<GrbRows> out;
+	for (const GrbRows &r : rows)
+	{
+		if (r.y1 <= r.y0)
+			continue;
+		if (!out.empty() && r.y0 <= out.back().y1)
+			out.back().y1 = std::max(out.back().y1, r.y1);
+		else
+			out.push_back(r);
+	}
+	return out;
+}
+
+// The rows of `set` (disjoint ranges in increasing order) inside `with`.
+std::vector<GrbRows> intersect(const std::vector<GrbRows> &set, GrbRows with)
+{
+	std::vector<GrbRows> out;
+	for (const GrbRows &r : set)
+	{
+		const int y0 = std::max(r.y0, with.y0), y1 = std::min(r.y1, with.y1);
+		if (y1 > y0)
+			out.push_back(GrbRows{ y0, y1 });
+	}
+	return out;
+}
+} // namespace
+
+GrbRows cluster_tile_rows(int y0, int y1, int height, int resolution_y)
+{
+	int t0 = int((long long)y0 * (long long)resolution_y / height) - 1;
+	int t1 = int(((long long)y1 * (long long)resolution_y + height - 1) / height) + 1;
+	return GrbRows{ std::max(t0, 0), std::min(t1, resolution_y) };
+}
+
+StripePlan compute_stripe_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality,
+                               bool taa, unsigned stripe_rows, unsigned cluster_rows)
+{
+	if (stripe_rows == 0 || stripe_rows % 8 != 0)
+		throw std::invalid_argument("lighting stripes must be a positive multiple of 8 rows (got " + std::to_string(stripe_rows) + ")");
+	StripePlan sp;
+	const unsigned world = std::max<unsigned>((unsigned)bands.size(), 1u);
+	for (unsigned y = rank * stripe_rows; y < height; y += world * stripe_rows)
+		sp.lit.push_back(GrbRows{ (int)y, (int)std::min(y + stripe_rows, height) });
+	sp.push.resize(world);
+	const GrbRows own_lighting = compute_shard_plan(width, height, bands, rank, fxaa, smaa_quality, taa).lighting;
+	if (world > 1)
+		for (unsigned q = 0; q < world; q++)
+			if (q != rank)
+				sp.push[q] = intersect(sp.lit, compute_shard_plan(width, height, bands, q, fxaa, smaa_quality, taa).lighting);
+	// L_r minus S_r
+	int y = own_lighting.y0;
+	for (const GrbRows &r : intersect(sp.lit, own_lighting))
+	{
+		if (r.y0 > y)
+			sp.receive.push_back(GrbRows{ y, r.y0 });
+		y = r.y1;
+	}
+	if (y < own_lighting.y1)
+		sp.receive.push_back(GrbRows{ y, own_lighting.y1 });
+	std::vector<GrbRows> all = sp.lit;
+	all.push_back(own_lighting);
+	sp.upload = merged(all);
+	std::vector<GrbRows> tiles;
+	for (const GrbRows &r : sp.lit)
+		tiles.push_back(cluster_tile_rows(r.y0, r.y1, (int)height, (int)cluster_rows));
+	sp.tile_rows = merged(tiles);
+	return sp;
+}
+
 void check_band_layout(unsigned width, unsigned height, const std::vector<GrbRows> &bands, ShardUpscale upscale)
 {
 	int expect = 0;

@@ -113,6 +113,31 @@ struct ShardUpscale
 ShardPlan compute_shard_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality = -1,
                              bool taa = false, ShardUpscale upscale = {});
 
+// Lighting in stripes (opt-in): rank r of W lights the stripes k with k mod W == r, rows [k s, min((k + 1) s, H)) for
+// stripes of s rows, whatever the bands; the bands still decide who runs the post chain on which rows (the plan above,
+// unchanged).  A rank then holds the HDR rows of its lighting rows L_r that it lit itself and receives the others from
+// the ranks that lit them.  Lighting is per pixel and a light that cannot reach a pixel adds exactly 0, so any split of
+// the rows gives the unsharded image bit for bit.
+struct StripePlan
+{
+	std::vector<GrbRows> lit;               // S_r: this rank's stripes, clipped to the image
+	std::vector<std::vector<GrbRows>> push; // [q]: the rows of S_r inside rank q's lighting rows L_q (none for q = rank)
+	std::vector<GrbRows> receive;           // the rows of L_r that other ranks light
+	std::vector<GrbRows> upload;            // S_r u L_r, merged: the G-buffer rows that must be resident
+	std::vector<GrbRows> tile_rows;         // cluster tile-row ranges the lighting of S_r reads (cluster_tile_rows per stripe, merged)
+};
+
+// The stripe plan of `rank` for stripes of stripe_rows rows (a positive multiple of 8) with the same bands and post
+// chain as compute_shard_plan, and a light cluster of cluster_rows tile rows.  Unsharded (one band): the whole image.
+// Throws std::invalid_argument for a bad stripe height.
+StripePlan compute_stripe_plan(unsigned width, unsigned height, const std::vector<GrbRows> &bands, unsigned rank, bool fxaa, int smaa_quality,
+                               bool taa, unsigned stripe_rows, unsigned cluster_rows);
+
+// The cluster tile rows under pixel rows [y0, y1) of a frame `height` rows tall with `resolution_y` tile rows: a tile
+// row of a pixel row is floor((y + 0.5) / height * resolution_y) (clustering.frag through clusterer_bindless.h:29-40);
+// one tile row of margin either side covers the rounding of that product.
+GrbRows cluster_tile_rows(int y0, int y1, int height, int resolution_y);
+
 // A new layout for moving the cuts of a sharded frame: throws std::invalid_argument unless `bands` tile [0, height) in
 // order, or (under FSR 1) when a rank would produce no render rows.
 void check_band_layout(unsigned width, unsigned height, const std::vector<GrbRows> &bands, ShardUpscale upscale);

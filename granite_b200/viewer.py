@@ -270,6 +270,26 @@ def shard_plan_fsr(width, height, render_width, render_height, bands, rank, post
     return {k: (out[i].y0, out[i].y1) for i, k in enumerate(FSR_PLAN_FIELDS)}
 
 
+def shard_plan_stripes(width, height, bands, rank, stripe_rows, post_aa=AA_NONE, cluster_rows=64) -> dict:
+    """Rows of one rank of a row-sharded frame that lights in stripes of `stripe_rows` rows (host math of
+    granite_b200/host/shard_plan.cpp): `lit` (its stripes), `receive` (its lighting rows that other ranks light),
+    `upload` (the G-buffer rows it must hold), `tile_rows` (the cluster tile rows its stripes read) as lists of
+    (y0, y1), and `push` (per rank q, the rows of its stripes inside q's lighting rows).  cluster_rows: the light
+    cluster's tile rows (the viewer's cluster_res[1])."""
+    world = max(len(bands), 1)
+    arr = (capi.GrbRows * world)(*[capi.GrbRows(a, b) for a, b in bands])
+    capacity = (world + 4) * (height // 8 + 2)
+    out = (capi.GrbRows * capacity)()
+    counts = (C.c_int32 * (world + 4))()
+    _check(lib().grbh_shard_plan_stripes(width, height, arr, len(bands), rank, int(post_aa), int(stripe_rows), int(cluster_rows), out, capacity,
+                                         counts), "grbh_shard_plan_stripes")
+    lists, at = [], 0
+    for n in counts:
+        lists.append([(out[i].y0, out[i].y1) for i in range(at, at + n)])
+        at += n
+    return {"lit": lists[0], "receive": lists[1], "upload": lists[2], "tile_rows": lists[3], "push": lists[4:]}
+
+
 class Viewer:
     def __init__(self, width, height, post_aa=AA_NONE, hdr_bloom=True, dynamic_exposure=True, cuda_device=0,
                  cluster_res=(128, 64, 4096), timestamps=False, stream=None, pipelined_io=False, hdr10_output=False, hdr10_max_cll=1000.0,
@@ -376,6 +396,11 @@ class Viewer:
     def set_row_shards(self, bands, rank):
         arr = (capi.GrbRows * len(bands))(*[capi.GrbRows(a, b) for a, b in bands])
         _check(lib().grbh_viewer_set_row_shards(self._h, arr, len(bands), rank), "grbh_viewer_set_row_shards")
+
+    def set_lighting_stripes(self, rows):
+        """Row-sharded frames: light interleaved stripes of `rows` rows (a positive multiple of 8; 0 = off) on every rank
+        instead of each rank's band (grbh_viewer_set_lighting_stripes).  Before bake; the same value on every rank."""
+        _check(lib().grbh_viewer_set_lighting_stripes(self._h, int(rows)), "grbh_viewer_set_lighting_stripes")
 
     def set_present_rank(self, rank):
         """Present row-sharded frames from `rank` (-1: off): read_output / read_output_async there return the whole

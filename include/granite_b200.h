@@ -254,6 +254,25 @@ typedef struct GrbLightShadows
 	int32_t pcf_wide;   /* != 0: SHADOW_MAP_PCF_KERNEL_WIDE (config "PCFKernelWide", renderer.cpp:380-381): spot lights filter with the
 	                     * 6 x 6 kernel of pcf.h:7-80 instead of the sampler's 2 x 2; point lights keep the cube sampler */
 } GrbLightShadows;
+/* A stripe set: the rows [first + k * period, first + k * period + rows) for k = 0, 1, ..., clipped to the image.  A
+ * row-sharded frame that lights in stripes gives rank r of W the set {r * s, s, W * s} for stripes of s rows. */
+typedef struct GrbStripes
+{
+	int32_t first, rows, period;
+} GrbStripes;
+/* The lighting pass over a stripe set instead of one band of rows: every pixel of the set gets what grb_deferred_lighting
+ * of the whole image writes there, bit for bit (a light that cannot reach a pixel adds exactly 0), and no other pixel is
+ * written.  The persistent form (the one grb_deferred_lighting_scheduled runs) lights the whole set in one launch, its
+ * 4-row work items taken from the set; `schedule` (grb_lighting_schedule_bytes(image height) bytes, as for
+ * grb_deferred_lighting_scheduled, or NULL) then orders the set's strips and is reset when the set's strip count
+ * changes.  The other forms (R16G16B16A16_SFLOAT hdr, shadowed lights, odd widths) run one launch per stripe.
+ * shadows: NULL for unshadowed lights, else as grb_deferred_lighting_shadowed.
+ * GRB_ERR_INVALID_ARGUMENT: first < 0, rows not a positive multiple of 4, period < rows, or an argument
+ * grb_deferred_lighting(_shadowed) refuses; GRB_ERR_UNSUPPORTED_FORMAT as grb_deferred_lighting. */
+int32_t grb_deferred_lighting_stripes(const GrbGBuffer *gbuffer, const GrbCamera *cam, const GrbClusterParameters *params,
+                                      const GrbClusterBuffers *buf, const GrbLightShadows *shadows, const GrbImage *hdr, GrbStripes stripes,
+                                      void *schedule, void *stream);
+
 /* The lighting pass with shadowed positional lights; every other argument as grb_deferred_lighting. */
 int32_t grb_deferred_lighting_shadowed(const GrbGBuffer *gbuffer, const GrbCamera *cam, const GrbClusterParameters *params,
                                        const GrbClusterBuffers *buf, const GrbLightShadows *shadows, const GrbImage *hdr, GrbRows rows,
@@ -444,6 +463,20 @@ int32_t grb_taa_resolve_to_peers(const GrbImage *hdr, const GrbImage *depth, con
  * (the reference never splits a frame). */
 int32_t grb_present_rows_to_peer(const GrbImage *src, void *dst, uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch,
                                  uint32_t *scratch_counter, GrbRows own, void *stream);
+/* Lighting in stripes on a row-sharded frame: the rank that lit the stripe set `stripes` (grb_deferred_lighting_stripes)
+ * stores each of its rows that lies in rank q's lighting rows peer_rows[q] into peer_images[q], for every q other than
+ * flag_index.  peer_images[q] is the base address, valid on this device, of rank q's HDR slot (cudaIpc-mapped peer
+ * memory) with hdr's size and pitch; the rows keep their place.  Texels of 4 or 8 bytes (B10G11R11_UFLOAT or
+ * R16G16B16A16_SFLOAT), 16-byte stores when the pitch and every base allow it.  Then flags[flag_index] = epoch is
+ * release-stored into the flag array of EVERY rank, also when no row went anywhere; the consumer is grb_peer_wait on all
+ * peer_count flags before it reads its slot.  scratch_counter: one zero-initialised uint32 in local device memory.
+ * GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, a
+ * texel size other than 4 or 8 bytes, more than 65535 rows, first < 0, rows < 1, period < rows, a peer_rows entry that is not a range inside
+ * the image (empty allowed), another rank's slot equal to hdr->data (checked before any CUDA call; nothing is written).
+ * No reference equivalent (the reference never splits a frame). */
+int32_t grb_hdr_rows_to_peers(const GrbImage *hdr, void *const *peer_images, uint32_t *const *peer_flags, const GrbRows *peer_rows,
+                              int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, GrbStripes stripes,
+                              void *stream);
 
 #ifdef __cplusplus
 }

@@ -140,6 +140,15 @@ int32_t grbh_viewer_set_row_shards(GrbhViewer *viewer, const GrbRows *bands, int
  * Every rank must set the same value.  Must precede bake.  Readers of the presented frame must be stream-ordered
  * behind the frame (these readbacks are): DESIGN.md section 5, "Presenting a sharded frame". */
 int32_t grbh_viewer_set_present_rank(GrbhViewer *viewer, int32_t rank);
+/* Row-sharded frames lit in stripes of stripe_rows rows (a positive multiple of 8; 0 = off, the default): rank r of W
+ * lights the stripes k with k mod W == r, rows [k * stripe_rows, min((k + 1) * stripe_rows, height)), whatever the
+ * bands, so every rank gets its share of the light-dense and of the sparse rows without a measurement.  Each rank then
+ * pushes the rows other ranks' lighting rows hold into their HDR-main (through NVLink peer memory, or NCCL broadcasts
+ * without it), and a "lighting-exchange" pass after "lighting" waits for them.  The bands keep deciding who runs the
+ * post chain on which rows; grbh_viewer_move_row_shards and grbh_viewer_set_present_rank work unchanged.  Call before
+ * grbh_viewer_bake, with the same value on every rank.  The frame equals the unsharded frame bit for bit.  Refused under
+ * FSR 1 (resolution_scale < 1) and for a value that is not a multiple of 8; on an unsharded viewer it changes nothing. */
+int32_t grbh_viewer_set_lighting_stripes(GrbhViewer *viewer, int32_t stripe_rows);
 /* Moves the band cuts of a baked row-sharded viewer; takes effect from the next grbh_viewer_render_frame.
  * bands: `count` rows ranges that tile [0, height) in order, count = the band count the viewer was baked with; the rank
  * stays.  Under FSR 1 a layout in which some rank would produce no render rows is refused, as by
@@ -187,6 +196,23 @@ int32_t grbh_shard_plan_taa(int32_t width, int32_t height, const GrbRows *bands,
  * Whole images when count <= 1.  Fails when some rank would produce no render rows.  Pure host math. */
 int32_t grbh_shard_plan_fsr(int32_t width, int32_t height, int32_t render_width, int32_t render_height, const GrbRows *bands, int32_t count,
                             int32_t rank, int32_t post_aa, int32_t rcas, GrbRows *out12);
+
+/* The rows of one rank of a row-sharded frame that lights in stripes of stripe_rows rows (a positive multiple of 8):
+ * rank r of `count` lights the stripes k with k mod count == r, rows [k * stripe_rows, min((k + 1) * stripe_rows,
+ * height)), whatever the bands; the bands and post_aa (a GrbhPostAA) give every rank's lighting rows L_q as in
+ * grbh_shard_plan / _smaa / _taa.  cluster_rows: the light cluster's tile rows.  The ranges go to `out` list after list,
+ * and counts[i] receives the length of list i:
+ *   0  lit:       the rank's stripes S_r, clipped to the image
+ *   1  receive:   the rows of L_r that other ranks light
+ *   2  upload:    S_r u L_r merged, the G-buffer rows that must be resident
+ *   3  tile rows: the cluster tile rows the lighting of S_r reads (the clusterer's pixel-row to tile-row rounding with
+ *                 one tile row of margin, per stripe, merged)
+ *   4 + q         push to q: the rows of S_r inside L_q (none for q = rank)
+ * counts holds max(count, 1) + 4 entries.  One band or none: the whole image, nothing pushed or received.  Returns the
+ * number of ranges; fails when that exceeds capacity, or for a stripe height that is not a positive multiple of 8.
+ * Pure host math. */
+int32_t grbh_shard_plan_stripes(int32_t width, int32_t height, const GrbRows *bands, int32_t count, int32_t rank, int32_t post_aa,
+                                int32_t stripe_rows, int32_t cluster_rows, GrbRows *out, int32_t capacity, int32_t *counts);
 
 /* bake_render_graph: declares the passes, bakes, allocates attachments. */
 int32_t grbh_viewer_bake(GrbhViewer *viewer);
