@@ -218,17 +218,21 @@ def _per_pixel_sum(pix, v, n):
 
 
 # ----------------------------------------------------------------------------------------------- reference + bar
-def reference(oracle, scene, cam, prep, clus, indices=None, emissive=None):
+def reference(oracle, scene, cam, prep, clus, indices=None, emissive=None, pairs=None):
     """Float64 values and slacks of every lit pixel.  indices = (tile, zi) from oracle.deferred_lighting(...,
-    want_indices=True) (computed here when None); emissive: the destination's initial words (scene.emissive)."""
-    if indices is None:
-        _, tile, zi, _ = oracle.deferred_lighting(scene, cam, prep, clus, want_indices=True)
-    else:
-        tile, zi = indices
+    want_indices=True) (computed here when None); emissive: the destination's initial words (scene.emissive).
+    pairs: draw 2's (pixel, light) pairs over the lit pixels in row-major order, in place of the cluster's (clus and
+    indices are then not read); tests/cluster_cases.py brute_pairs gives the pairs whose falloff is nonzero."""
     emissive = scene.emissive if emissive is None else emissive
     lit = scene.depth != 0
     ys, xs = np.nonzero(lit)
-    pairs = light_pairs(prep, clus, tile, zi, ys, xs)
+    tile = zi = None
+    if pairs is None:
+        if indices is None:
+            _, tile, zi, _ = oracle.deferred_lighting(scene, cam, prep, clus, want_indices=True)
+        else:
+            tile, zi = indices
+        pairs = light_pairs(prep, clus, tile, zi, ys, xs)
     srgb = srgb_table(oracle)
     d64, t64 = evaluate(scene, cam, prep, pairs, ys, xs, srgb, "ref", np.float64)
     d32, t32 = evaluate(scene, cam, prep, pairs, ys, xs, srgb, "ref", np.float32)

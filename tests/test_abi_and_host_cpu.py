@@ -134,29 +134,44 @@ def test_host_camera_block(built, oracle):
     assert cam.z_near == ref.z_near and cam.z_far == pytest.approx(ref.z_far, rel=1e-6)
 
 
-@pytest.mark.parametrize("n,spots", [(0, 0.0), (16, 0.0), (300, 0.25), (4096, 0.25)])
-def test_host_light_prep_is_byte_identical_to_oracle(built, oracle, n, spots):
-    from granite_b200 import synth
-    from tests import common
+@pytest.mark.parametrize("case", [pytest.param((n, s), id=f"{n}-{s}") for n, s in [(0, 0.0), (16, 0.0), (300, 0.25), (4096, 0.25)]]
+                         + [pytest.param(name, id=name) for name in ("turned", "around-eye", "spots-at-eye", "finite-far", "tall")])
+def test_host_light_prep_is_byte_identical_to_oracle(built, oracle, case):
+    """The host LightClusterer's prep (frustum culling, front-to-back order, records, model rows, type mask, Z-slice
+    ranges) byte for byte the oracle's, on the default view and on the geometry cases of tests/cluster_cases.py (turned
+    cameras, a finite far plane, lights at, behind and beside the eye), each set through Viewer.set_camera."""
+    from granite_b200 import synth, viewer
+    from tests import cluster_cases, common
 
-    v = _host_viewer()
-    lights = synth.make_lights(n, spot_fraction=spots)
+    if isinstance(case, str):
+        scene, _, lights, _ = cluster_cases.build(oracle, case, check=False)
+        v = viewer.Viewer(scene.width, scene.height, cuda_device=-1)
+        v.set_camera(scene.projection, scene.view)
+    else:
+        v = _host_viewer()
+        lights = synth.make_lights(case[0], spot_fraction=case[1])
+    n = len(lights.color)
     # hand the lights over in a shuffled order: the clusterer must restore front-to-back order
     perm = np.random.default_rng(1).permutation(n)
     shuffled = synth.Lights(lights.color[perm], lights.position[perm], lights.is_point[perm], lights.rot[perm],
                             lights.inner_cone[perm], lights.outer_cone[perm])
     v.set_lights(shuffled)
     k, recs, model, tmask, zr = v.light_prep()
-    assert k == n
     cam = common.oracle_camera_from_viewer(oracle, v)
     prep = oracle.prepare_lights(cam, lights)
-    assert recs.tobytes() == prep.records[:n].tobytes()
-    assert np.array_equal(model.view(np.uint32), prep.model[:n].view(np.uint32))
+    assert k == prep.n and (k == n or isinstance(case, str))
+    assert recs.tobytes() == prep.records[:k].tobytes()
+    assert np.array_equal(model.view(np.uint32), prep.model[:k].view(np.uint32))
     assert np.array_equal(tmask, prep.type_mask[: len(tmask)])
     assert np.array_equal(zr, prep.z_ranges)
     p = prep.params
-    # ClustererParametersBindless: z_scale = 1 / min(0.5, z_far / res_z) = 2, 128x64 tiles
-    assert p.z_scale == 2.0 and p.z_max_index == 4095 and list(p.resolution_xy) == [128, 64] and p.num_lights_32 == (n + 31) // 32
+    # ClustererParametersBindless: z_scale = 1 / min(0.5, z_far / res_z), 128x64 tiles
+    z_scale = np.float32(1.0) / min(np.float32(0.5), np.float32(cam.z_far) / np.float32(4096))
+    assert p.z_scale == z_scale and p.z_max_index == 4095 and list(p.resolution_xy) == [128, 64] and p.num_lights_32 == (k + 31) // 32
+    if not isinstance(case, str):
+        assert p.z_scale == 2.0
+    elif case == "finite-far":
+        assert p.z_scale > 30.0 and (zr[:, 1] == 4095).any(), "slices end at the far plane"
 
 
 def test_hdr10_output_rejects_fxaa(built):

@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import common
+from tests import cluster_cases, common
 
 pytestmark = pytest.mark.gpu
 
@@ -24,13 +24,6 @@ CONFIGS = [
 C3 = pytest.param(3840, 2160, 4096, 0.0, id="C3-4K-4096pt")
 
 
-def _canon(a):
-    """fp32 bit patterns with every NaN mapped to one pattern (x86 and NVIDIA differ in the
-    default NaN they generate; any NaN compares the same way in the shaders)."""
-    a = np.ascontiguousarray(a, np.float32)
-    return np.where(np.isnan(a), np.uint32(0x7FC00000), a.view(np.uint32))
-
-
 def _cluster(cuda, oracle, cam, prep):
     from granite_b200 import harness
 
@@ -41,50 +34,44 @@ def _cluster(cuda, oracle, cam, prep):
     return dev, gcam
 
 
-@pytest.mark.parametrize("w,h,n,spots", CONFIGS + [pytest.param(3840, 2160, 4096, 0.25, id="C3-4096-25pct-spots")])
-def test_cluster_build_bit_exact(cuda, oracle, w, h, n, spots):
-    cam, lights, prep = common.build_lights_case(oracle, w / h, n, spots)  # the clusterer does not read the G-buffer
+# the default view at the configurations above, and the geometry cases of tests/cluster_cases.py (turned cameras,
+# lights at and behind the eye, a finite far plane, a tall wide-angle view)
+_GEOMETRY = [pytest.param(name, id=name) for name in cluster_cases.CASES]
+
+
+def _config(p):
+    return pytest.param(p.values, id=p.id)
+
+
+def _lights_case(oracle, case):
+    """(cam, prep) of a default-view configuration (w, h, n, spots) or a named geometry case."""
+    if isinstance(case, str):
+        _, cam, _, prep = cluster_cases.build(oracle, case)
+        return cam, prep
+    w, h, n, spots = case
+    cam, _, prep = common.build_lights_case(oracle, w / h, n, spots)  # the clusterer does not read the G-buffer
+    return cam, prep
+
+
+@pytest.mark.parametrize("case", [_config(p) for p in CONFIGS + [pytest.param(3840, 2160, 4096, 0.25, id="C3-4096-25pct-spots")]] + _GEOMETRY)
+def test_cluster_build_bit_exact(cuda, oracle, case):
+    cam, prep = _lights_case(oracle, case)
     ref = oracle.cluster_build(cam, prep)
     dev, _ = _cluster(cuda, oracle, cam, prep)
-    got = dev.download()
-    is_point = np.array([(prep.type_mask[i >> 5] >> (i & 31)) & 1 for i in range(n)], bool)
-    # K1: spot hull (only spot entries are consumed)
-    assert np.array_equal(_canon(got.spots[:n][~is_point]), _canon(ref.spots[:n][~is_point]))
-    # K2: point lights use data[0..3]; spots use 4 vec4 per emitted triangle (+ count in data[0].w)
-    assert np.array_equal(_canon(got.cull[:n][is_point][:, :16]), _canon(ref.cull[:n][is_point][:, :16]))
-    for i in np.nonzero(~is_point)[0]:
-        cnt = int(ref.cull[i].view(np.uint32)[3])
-        assert int(got.cull[i].view(np.uint32)[3]) == cnt
-        used = 16 * min(cnt, 8) if cnt <= 8 else 0
-        a, b = _canon(got.cull[i][:used]).copy(), _canon(ref.cull[i][:used]).copy()
-        if used:
-            a[3] = b[3] = 0
-        assert np.array_equal(a, b), f"spot {i}"
-    # K3 / K4: the integer contract
-    assert np.array_equal(got.bitmask, ref.bitmask)
-    assert np.array_equal(got.range, ref.range)
-    # bits >= num_lights are zero
-    if n % 32:
-        assert not (got.bitmask[..., -1] >> np.uint32(n % 32)).any()
+    cluster_cases.assert_cluster_equal(dev.download(), ref, prep)
 
 
-@pytest.mark.parametrize("w,h,n,spots", CONFIGS + [C3])
-def test_cluster_indices_bit_exact(cuda, oracle, w, h, n, spots):
-    from granite_b200 import capi, harness
-
-    scene, cam, lights, prep = common.build_case(oracle, w, h, n, spots)
+@pytest.mark.parametrize("case", [_config(p) for p in CONFIGS + [C3]] + _GEOMETRY)
+def test_cluster_indices_bit_exact(cuda, oracle, case):
+    if isinstance(case, str):
+        scene, cam, _, prep = cluster_cases.build(oracle, case)
+    else:
+        scene, cam, _, prep = common.build_case(oracle, *case)
     clus = oracle.cluster_build(cam, prep)
     _, tile, zi, _ = oracle.deferred_lighting(scene, cam, prep, clus, want_indices=True)
-    depth = harness.to_dev(scene.depth)
-    out_t = torch.zeros((h, w), dtype=torch.int32, device="cuda")
-    out_z = torch.zeros((h, w), dtype=torch.int32, device="cuda")
-    img = capi.image(depth, capi.FORMAT_D32_SFLOAT)
-    gcam = harness.camera_struct(cam)
-    params = harness.params_struct(prep.params)
-    capi.check(capi.lib().grb_debug_cluster_indices(C.byref(img), C.byref(gcam), C.byref(params), C.c_void_p(out_t.data_ptr()),
-                                                    C.c_void_p(out_z.data_ptr()), capi.rows(), capi.stream_ptr()))
-    assert np.array_equal(out_t.cpu().numpy(), tile)
-    assert np.array_equal(out_z.cpu().numpy(), zi)
+    got_t, got_z = cluster_cases.debug_cluster_indices(cam, prep, scene.depth)
+    assert np.array_equal(got_t, tile)
+    assert np.array_equal(got_z, zi)
 
 
 @pytest.mark.parametrize("w,h,n,spots", [pytest.param(640, 360, 300, 0.25, id="small-300-25pct-spots"), pytest.param(322, 190, 100, 0.0, id="ragged-322x190")])
