@@ -715,9 +715,8 @@ struct PersistentArgs
 	QueueSlot *queue;
 	int blocks_x, blocks_y, total_items; // total_items = blocks_x * blocks_y
 	int n_lights;
-	uint32_t *schedule; // optional: [blocks_x, blocks_y, valid, 0][max block cost per strip][strips by falling cost][block shape per strip]
+	uint32_t *schedule; // optional: [blocks_x, blocks_y, valid, 0][max block cost per strip][strips by falling cost]
 	unsigned rec_bytes; // n_lights * 48, multiple of 16
-	unsigned row_shape_threshold; // 0 = every strip uses 16x4 blocks (default); else cost (cycles >> 5) above which a strip switches to 64x1 blocks
 };
 
 struct SurfaceP
@@ -833,10 +832,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 	                       a.schedule[1] == (uint32_t)a.blocks_y && a.schedule[2] == 1u;
 	if (scheduled)
 		for (int i = threadIdx.x; i < a.blocks_y; i += blockDim.x)
-		{
-			const uint32_t strip = a.schedule[4 + a.blocks_y + i];
-			s_order[i] = (uint16_t)(strip | (a.schedule[4 + 2 * a.blocks_y + strip] ? 0x8000u : 0u));
-		}
+			s_order[i] = (uint16_t)a.schedule[4 + a.blocks_y + i];
 	__syncthreads();
 	// the light table (16-byte aligned, launch_deferred_lighting checks it) by the bulk-copy engine
 	if (threadIdx.x == 0 && a.rec_bytes)
@@ -859,23 +855,13 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 	const unsigned total = (unsigned)a.total_items;
 	const unsigned n_warps = gridDim.x * kPWarps;
 
-	// Work items are pixel blocks, strip by strip (a strip = 4 pixel rows) in schedule order, one item per
-	// atomic.  A strip is cut into blocks in one of two shapes, chosen per strip from the previous
-	// launch's costs (bit 15 of its s_order entry):
-	//   shape 0: 16 x 4 pixels (lane = 8 x 4 pixel pairs)      -- compact footprint, one or two cluster tiles
-	//   shape 1: 64 x 1 pixels (lane = 32 pixel pairs of a row) -- for the light-dense strips near the
-	//            horizon, where depth changes by metres from one pixel row to the next: a 4-row block's
-	//            bounding box then collects several times the lights any of its pixels sees, a single
-	//            row's does not.
-	// Either way a strip has a.blocks_x = 4 * ceil(w / 64) items (>= ceil(w / 16); surplus shape-0 items are
-	// empty).  Per-pixel results do not depend on the shape: a light that does not reach a pixel adds 0.
+	// Work items are 16x4-pixel blocks (lane = 8 x 4 pixel pairs), a.blocks_x = ceil(w / 16) per strip (4 pixel
+	// rows), strip by strip in schedule order, one item per atomic.
 	//
 	// The atomic for the NEXT item is normally issued when the current one is taken (its round trip and
 	// the G-buffer prefetch overlap the current block's shading).  After a block with a long light list
 	// the warp stops reserving ahead: a reserved block is a block no idle warp can take, and a dense
 	// block can take 100 us.
-	const unsigned n64 = (unsigned)a.blocks_x / 4u;
-	const unsigned blocks16 = ((unsigned)p.hdr.w / 2u + 7u) / 8u;
 	unsigned pend_got = 0;
 	bool pending = false, dense_mode = false;
 	auto issue_grab = [&]() {
@@ -887,7 +873,6 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 	{
 		int x, y;       // this lane's pixel pair
 		int px0, py0;   // first pixel of the block
-		int pw, ph;     // its extent
 		int strip;
 	};
 	auto fetch_item = [&](Item &it) -> bool {
@@ -910,27 +895,11 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 #endif
 		const unsigned row = item / (unsigned)a.blocks_x;
 		const unsigned i = item - row * (unsigned)a.blocks_x;
-		const unsigned enc = scheduled ? (unsigned)s_order[row] : row;
-		it.strip = (int)(enc & 0x7fffu);
-		if (enc & 0x8000u)
-		{
-			const unsigned r = i / n64, bx = i - r * n64;
-			it.px0 = (int)bx * 64;
-			it.py0 = strips.first_row(p, it.strip) + (int)r;
-			it.pw = 64;
-			it.ph = 1;
-			it.x = it.px0 + 2 * lane;
-			it.y = it.py0;
-		}
-		else
-		{
-			it.px0 = i < blocks16 ? (int)i * 16 : p.hdr.w; // surplus items lie outside the image
-			it.py0 = strips.first_row(p, it.strip);
-			it.pw = 16;
-			it.ph = 4;
-			it.x = it.px0 + 2 * (lane & 7);
-			it.y = it.py0 + (lane >> 3);
-		}
+		it.strip = scheduled ? (int)s_order[row] : (int)row;
+		it.px0 = (int)i * 16;
+		it.py0 = strips.first_row(p, it.strip);
+		it.x = it.px0 + 2 * (lane & 7);
+		it.y = it.py0 + (lane >> 3);
 		return true;
 	};
 	// The G-buffer words of the NEXT block are copied asynchronously (cp.async, no registers held)
@@ -1055,7 +1024,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 			if (lo <= hi) // otherwise empty slices only: (0xffffffff, 0)
 			{
 				const int px0 = cur.px0, py0 = cur.py0; // the block's first pixel
-				const int px1 = min(px0 + cur.pw - 1, p.hdr.w - 1), py1 = min(py0 + cur.ph - 1, p.y1 - 1);
+				const int px1 = min(px0 + 15, p.hdr.w - 1), py1 = min(py0 + 3, p.y1 - 1);
 				const int tx0 = cluster_tile_x(p, px0), tx1 = cluster_tile_x(p, px1), ty0 = cluster_tile_y(p, py0), ty1 = cluster_tile_y(p, py1);
 				// cluster_mask_range (clusterer_bindless_buffers.h:17-27) for a warp-uniform range: only the
 				// first and the last word of [lo, hi] are cut
@@ -1220,7 +1189,7 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 #ifdef GRB_LIGHTING_DEBUG
 		if (lane == 0)
 		{
-			const int bi = cur_by * a.blocks_x + (cur.ph == 4 ? (cur.px0 >> 4) : ((cur.py0 - strips.first_row(p, cur_by)) * (a.blocks_x / 4) + (cur.px0 >> 6)));
+			const int bi = cur_by * a.blocks_x + (cur.px0 >> 4);
 			if (bi < kDbgBlocks)
 				g_dbg_block[bi] = make_uint2((uint32_t)(clock64() - t_begin), (uint32_t)(globaltimer_ns() - s_t0));
 		}
@@ -1273,13 +1242,6 @@ __global__ void __launch_bounds__(32 * kPWarps, 1) deferred_lighting_persistent_
 			}
 			a.schedule[4 + a.blocks_y + rank] = (uint32_t)i;
 			a.schedule[4 + i] = 0u;
-			// block shape of strip i for the next launch (only when the experiment is switched on, see
-			// PersistentArgs::row_shape_threshold): one-row blocks once its most expensive block exceeds the
-			// threshold, back to 16x4 only when it falls below a quarter of that (the measure itself
-			// depends on the shape: no flip-flopping)
-			const uint32_t old_shape = a.schedule[4 + 2 * a.blocks_y + i];
-			a.schedule[4 + 2 * a.blocks_y + i] =
-			    a.row_shape_threshold == 0u ? 0u : (mine > a.row_shape_threshold ? 1u : (mine < a.row_shape_threshold / 4u ? 0u : old_shape));
 		}
 		__syncthreads();
 		if (threadIdx.x == 0)
@@ -1421,7 +1383,7 @@ extern "C" int32_t grb_debug_lighting_dump2(void *items, void *last)
 extern "C" uint64_t grb_lighting_schedule_bytes(int32_t height)
 {
 	const uint64_t rows = (uint64_t)((height > 0 ? height : 0) + 3) / 4;
-	return (4u + 3u * rows) * sizeof(uint32_t); // header, cost, order, block shape per strip
+	return (4u + 2u * rows) * sizeof(uint32_t); // header, cost and order per strip
 }
 
 extern "C" int32_t grb_deferred_lighting(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params, const GrbClusterBuffers *buf,
@@ -1440,13 +1402,11 @@ extern "C" int32_t grb_deferred_lighting_scheduled(const GrbGBuffer *g, const Gr
 	return launch_deferred_lighting(g, cam, params, buf, hdr, rows, schedule, stream, false);
 }
 
-// The same pass as a plain grid of short-lived CTAs (one per 64x4 pixel block) instead of persistent ones.
-// For callers whose other streams must get SMs WHILE lighting runs: a persistent CTA keeps its SM (all of
-// its registers and shared memory) until the work queue is empty, so kernels of other streams that become
-// runnable in the meantime wait for the whole pass -- measured on a frame split over 2 GPUs, where the
-// post chain waits for the peer's band: 2441 frames/s with the persistent kernel, 3321 with this one.
-// Results are within the same parity bar; the two forms associate the per-light sums differently, so
-// they are not bit-identical to each other (use one form for every rank of a sharded frame).
+// The same pass as a plain grid of short-lived CTAs (the non-persistent pairs kernel, one CTA per 64x4 pixel
+// block; the one-pixel kernel where rows are not aligned pixel pairs) instead of persistent ones.  A persistent
+// CTA keeps its SM until the work queue is empty; these free their SMs as they finish.  Results are within the
+// same parity bar; the two forms associate the per-light sums differently, so they are not bit-identical to
+// each other.
 extern "C" int32_t grb_deferred_lighting_blocks(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params, const GrbClusterBuffers *buf,
                                                 const GrbImage *hdr, GrbRows rows, void *stream)
 {
@@ -1488,6 +1448,25 @@ extern "C" int32_t grb_deferred_lighting_stripes(const GrbGBuffer *g, const GrbC
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	return launch_deferred_lighting(g, cam, params, buf, hdr, GrbRows{ 0, 0 }, shadows ? nullptr : schedule, stream, shadows != nullptr, shadows, &stripes);
+}
+
+// What a pixel's position and (tile, Z slice) follow from: the camera, the cluster grid and the image size.
+static void set_cluster_geometry(LightingParams &p, const GrbCamera *cam, const GrbClusterParameters *params, int w, int h, GrbRows rows)
+{
+	for (int i = 0; i < 16; i++)
+		p.ivp[i] = cam->inv_view_projection[i];
+	p.cbase = make_float3(params->camera_base[0], params->camera_base[1], params->camera_base[2]);
+	p.cfront = make_float3(params->camera_front[0], params->camera_front[1], params->camera_front[2]);
+	p.xy_scale = make_float2(params->xy_scale[0], params->xy_scale[1]);
+	p.res_x = params->resolution_xy[0];
+	p.res_y = params->resolution_xy[1];
+	p.n32 = params->num_lights_32;
+	p.z_max_index = params->z_max_index;
+	p.z_scale = params->z_scale;
+	p.inv_res_x = 1.0f / (float)w; // renderer.cpp:1101-1102,1120
+	p.inv_res_y = 1.0f / (float)h;
+	p.y0 = rows.y0;
+	p.y1 = rows.y1;
 }
 
 static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *cam, const GrbClusterParameters *params, const GrbClusterBuffers *buf,
@@ -1556,27 +1535,14 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		p.emissive = view_of<const uint32_t>(hdr);
 		p.emissive16 = view_of<const uint2>(hdr);
 	}
-	for (int i = 0; i < 16; i++)
-		p.ivp[i] = cam->inv_view_projection[i];
+	set_cluster_geometry(p, cam, params, w, h, rows);
 	p.camera_pos = make_float3(cam->camera_position[0], cam->camera_position[1], cam->camera_position[2]);
 	p.dir_color = make_float3(g->directional_color[0], g->directional_color[1], g->directional_color[2]);
 	p.dir_dir = make_float3(g->directional_direction[0], g->directional_direction[1], g->directional_direction[2]);
-	p.cbase = make_float3(params->camera_base[0], params->camera_base[1], params->camera_base[2]);
-	p.cfront = make_float3(params->camera_front[0], params->camera_front[1], params->camera_front[2]);
-	p.xy_scale = make_float2(params->xy_scale[0], params->xy_scale[1]);
-	p.res_x = params->resolution_xy[0];
-	p.res_y = params->resolution_xy[1];
-	p.n32 = params->num_lights_32;
-	p.z_max_index = params->z_max_index;
-	p.z_scale = params->z_scale;
-	p.inv_res_x = 1.0f / (float)w; // renderer.cpp:1101-1102,1120
-	p.inv_res_y = 1.0f / (float)h;
 	p.lights = buf->lights;
 	p.type_mask = buf->type_mask;
 	p.bitmask = buf->bitmask;
 	p.cluster_range = reinterpret_cast<const uint2 *>(buf->cluster_range);
-	p.y0 = rows.y0;
-	p.y1 = rows.y1;
 	p.shadow_transforms = shadows ? shadows->transforms : nullptr;
 	p.shadow_maps = shadows ? reinterpret_cast<const uint16_t *const *>(shadows->maps) : nullptr;
 	p.shadow_res = shadows ? shadows->resolution : 0;
@@ -1628,7 +1594,7 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 			}
 		}
 		PersistentArgs a;
-		a.blocks_x = 4 * ((w + 63) / 64); // items per strip: 4 rows of 64x1 blocks, or ceil(w / 16) 16x4 blocks (+ empty ones)
+		a.blocks_x = (w + 15) / 16;
 		a.blocks_y = (rows.y1 - rows.y0 + 3) / 4;
 		StripeSetStrips strips = {};
 		if (stripes)
@@ -1643,12 +1609,6 @@ static int32_t launch_deferred_lighting(const GrbGBuffer *g, const GrbCamera *ca
 		a.schedule = static_cast<uint32_t *>(schedule);
 		a.n_lights = params->num_lights;
 		a.rec_bytes = (unsigned)params->num_lights * 48u;
-		{
-			// experiment, off by default: measured on the bench scene the one-row blocks execute 7 % MORE instructions (their
-			// lists are not shorter: depth varies along x as much as across 4 rows there) -- DESIGN.md section 4
-			static const char *e = getenv("GRB_LIGHTING_ROW_BLOCKS");
-			a.row_shape_threshold = e ? (unsigned)strtoul(e, nullptr, 10) : 0u;
-		}
 		a.queue = di.queue + (di.next_slot.fetch_add(1u, std::memory_order_relaxed) % 64u);
 		const size_t smem = (size_t)a.rec_bytes + 48u + 1024u + ((kPWarps * (kListCap + 2) * 2u + 15u) & ~15u) + 32u * kPWarps * kSlotBytes + 16u + kMaxOrderRows * 2u;
 		if (smem <= (size_t)di.smem_max)
@@ -1701,20 +1661,7 @@ extern "C" int32_t grb_debug_cluster_indices(const GrbImage *depth, const GrbCam
 		return GRB_OK;
 	LightingParams p{};
 	p.depth = view_of<const float>(depth);
-	for (int i = 0; i < 16; i++)
-		p.ivp[i] = cam->inv_view_projection[i];
-	p.cbase = make_float3(params->camera_base[0], params->camera_base[1], params->camera_base[2]);
-	p.cfront = make_float3(params->camera_front[0], params->camera_front[1], params->camera_front[2]);
-	p.xy_scale = make_float2(params->xy_scale[0], params->xy_scale[1]);
-	p.res_x = params->resolution_xy[0];
-	p.res_y = params->resolution_xy[1];
-	p.n32 = params->num_lights_32;
-	p.z_max_index = params->z_max_index;
-	p.z_scale = params->z_scale;
-	p.inv_res_x = 1.0f / (float)depth->width;
-	p.inv_res_y = 1.0f / (float)depth->height;
-	p.y0 = rows.y0;
-	p.y1 = rows.y1;
+	set_cluster_geometry(p, cam, params, depth->width, depth->height, rows);
 	dim3 grid((depth->width + 31) / 32, (rows.y1 - rows.y0 + 3) / 4, 1);
 	cluster_indices_kernel<<<grid, 128, 0, as_stream(stream)>>>(p, out_tile, out_z);
 	return check_launch("grb_debug_cluster_indices");
@@ -1750,23 +1697,10 @@ extern "C" int32_t grb_lighting_row_cost(const GrbImage *depth, const GrbCamera 
 	}
 	LightingParams p{};
 	p.depth = view_of<const float>(depth);
-	for (int i = 0; i < 16; i++)
-		p.ivp[i] = cam->inv_view_projection[i];
-	p.cbase = make_float3(params->camera_base[0], params->camera_base[1], params->camera_base[2]);
-	p.cfront = make_float3(params->camera_front[0], params->camera_front[1], params->camera_front[2]);
-	p.xy_scale = make_float2(params->xy_scale[0], params->xy_scale[1]);
-	p.res_x = params->resolution_xy[0];
-	p.res_y = params->resolution_xy[1];
-	p.n32 = params->num_lights_32;
-	p.z_max_index = params->z_max_index;
-	p.z_scale = params->z_scale;
-	p.inv_res_x = 1.0f / (float)depth->width;
-	p.inv_res_y = 1.0f / (float)depth->height;
+	set_cluster_geometry(p, cam, params, depth->width, depth->height, rows);
 	p.lights = buf->lights;
 	p.bitmask = buf->bitmask;
 	p.cluster_range = reinterpret_cast<const uint2 *>(buf->cluster_range);
-	p.y0 = rows.y0;
-	p.y1 = rows.y1;
 	const int pairs = (depth->width + 1) / 2;
 	dim3 grid((pairs + 8 * kWarpsPerCta - 1) / (8 * kWarpsPerCta), groups, 1);
 	lighting_cost_kernel<<<grid, 32 * kWarpsPerCta, 0, as_stream(stream)>>>(p, cost_per_4_rows);

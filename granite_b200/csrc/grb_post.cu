@@ -944,8 +944,6 @@ bool launch_tent_tiled(bool up, const GrbImage *in, const GrbImage *history, flo
 bool launch_tonemap_fast(const GrbImage *hdr, const GrbImage *bloom, const float *luminance, float exposure, const GrbImage *out, GrbRows rows, cudaStream_t stream,
                          int32_t *rc);
 bool launch_fxaa_fast(const GrbImage *in, const GrbImage *out, GrbRows rows, cudaStream_t stream, int32_t *rc);
-bool launch_taa_fast(const GrbImage *hdr, const GrbImage *depth, const GrbImage *mv, const GrbImage *history, const float *reproj16, const GrbImage *out_color,
-                     const GrbImage *out_history, GrbRows rows, cudaStream_t stream, int32_t *rc);
 } // namespace grb
 
 using namespace grb;
@@ -1353,18 +1351,9 @@ extern "C" int32_t grb_taa_resolve(const GrbImage *hdr, const GrbImage *depth, c
 		set_last_error("grb_taa_resolve: quality must be 0..2");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	// GRB_TAA_TILES=1 applies to whole-frame calls (rows {0, 0}) only: a row-sharded frame passes its rows and must
-	// compute the exact kernel's values, which grb_taa_resolve_to_peers computes on the other ranks
-	const bool whole_frame = rows.y0 == 0 && rows.y1 == 0;
 	rows = full_rows(rows, hdr->height);
 	if (rows.y1 <= rows.y0)
 		return GRB_OK;
-	if (history && quality == 2 && !hdr16 && whole_frame)
-	{
-		int32_t rc = GRB_OK;
-		if (launch_taa_fast(hdr, depth, mv, history, reproj16, out_color, out_history, rows, as_stream(stream), &rc))
-			return rc;
-	}
 	TaaInputs in{};
 	in.hdr = view_of<const uint32_t>(hdr);
 	Mat4 m{};

@@ -136,7 +136,7 @@ def deferred_lighting(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDe
 
 
 def deferred_lighting_blocks(gb: GBufferDevice, cam: capi.GrbCamera, cluster: ClusterDevice, hdr: torch.Tensor, rows=None):
-    """grb_deferred_lighting_blocks: the pass as a grid of short-lived CTAs (the form row-sharded frames may use)."""
+    """grb_deferred_lighting_blocks: the pass as a grid of short-lived CTAs (the non-persistent pairs kernel)."""
     img = _hdr_img(hdr)
     capi.check(capi.lib().grb_deferred_lighting_blocks(C.byref(gb.struct), C.byref(cam), C.byref(cluster.params), C.byref(cluster.buffers),
                                                        C.byref(img), capi.rows(rows), capi.stream_ptr()), "grb_deferred_lighting_blocks")

@@ -1,12 +1,11 @@
 #include "renderer.hpp"
 
-#include <cstdlib>
 #include <cstring>
 
 namespace Granite
 {
 void DeferredLightRenderer::render_light(Vulkan::CommandBuffer &cmd, const RenderContext &context, const GBufferViews &gb, Vulkan::ImageView &hdr,
-                                         GrbRows rows, void *schedule, bool blocks_form, const GrbStripes *stripes)
+                                         GrbRows rows, void *schedule, const GrbStripes *stripes)
 {
 	auto *light = context.get_lighting_parameters();
 	if (!light || !gb.albedo || !gb.normal || !gb.pbr || !gb.depth)
@@ -55,8 +54,6 @@ void DeferredLightRenderer::render_light(Vulkan::CommandBuffer &cmd, const Rende
 		return;
 	}
 	GrbImage hdr_img = hdr.as_grb();
-	// Row-sharded frames (rows != whole image, no schedule): the block form, so that the exchange-dependent
-	// post chain of the previous frame can interleave with this pass (see grb_deferred_lighting_blocks).
 	// POSITIONAL_LIGHTS_SHADOW (renderer.cpp:1124-1131): the clusterer holds the shadow transforms and map pointers
 	const GrbLightShadows shadows = light->cluster->get_light_shadows();
 	if (stripes)
@@ -65,8 +62,6 @@ void DeferredLightRenderer::render_light(Vulkan::CommandBuffer &cmd, const Rende
 		          "grb_deferred_lighting_stripes");
 	else if (shadows.maps)
 		cmd.check(grb_deferred_lighting_shadowed(&g, &cam, &params, &buffers, &shadows, &hdr_img, rows, cmd.get_stream_handle()), "grb_deferred_lighting_shadowed");
-	else if (blocks_form)
-		cmd.check(grb_deferred_lighting_blocks(&g, &cam, &params, &buffers, &hdr_img, rows, cmd.get_stream_handle()), "grb_deferred_lighting_blocks");
 	else
 		cmd.check(grb_deferred_lighting_scheduled(&g, &cam, &params, &buffers, &hdr_img, rows, schedule, cmd.get_stream_handle()), "grb_deferred_lighting");
 }
@@ -104,17 +99,12 @@ void DeferredLightingPass::build_render_pass(Vulkan::CommandBuffer &cmd)
 		gb.emissive = &graph->get_physical_texture_resource(*res_emissive);
 	auto &hdr = graph->get_physical_texture_resource(*res_hdr);
 	void *schedule = res_schedule ? graph->get_physical_buffer_resource(*res_schedule).get_device_pointer() : nullptr;
-	// GRB_SHARDED_BLOCKS=1: the block form of the kernel for row-sharded frames (many short CTAs instead of one
-	// persistent CTA per SM), as before the frame was phased.
-	static const bool sharded_blocks = getenv("GRB_SHARDED_BLOCKS") != nullptr;
-	const bool sharded = graph->is_sharded() && graph->get_shard_count() > 1;
 	if (push)
 	{
-		DeferredLightRenderer::render_light(cmd, context, gb, hdr, GrbRows{ 0, 0 }, schedule, false, &stripes);
+		DeferredLightRenderer::render_light(cmd, context, gb, hdr, GrbRows{ 0, 0 }, schedule, &stripes);
 		push(cmd, hdr);
 		return;
 	}
-	DeferredLightRenderer::render_light(cmd, context, gb, hdr, graph->is_sharded() ? graph->get_shard_plan().lighting : GrbRows{ 0, 0 }, schedule,
-	                                    sharded && sharded_blocks);
+	DeferredLightRenderer::render_light(cmd, context, gb, hdr, graph->is_sharded() ? graph->get_shard_plan().lighting : GrbRows{ 0, 0 }, schedule);
 }
 } // namespace Granite

@@ -26,12 +26,9 @@ class DeferredLightRenderer
 public:
 	// Adds directional + clustered lighting into `hdr` (in place; HDR-main aliases emissive).
 	// schedule: optional device buffer of grb_lighting_schedule_bytes(height) bytes kept across frames.
-	// blocks_form: the non-persistent kernel (grb_deferred_lighting_blocks) -- what a row-sharded frame uses
-	// on every rank, so that the post chain waiting for a peer's band can interleave with this pass.
 	// stripes: light that stripe set instead of `rows` (grb_deferred_lighting_stripes; row-sharded frames lit in stripes).
 	static void render_light(Vulkan::CommandBuffer &cmd, const RenderContext &context, const GBufferViews &gbuffer,
-	                         Vulkan::ImageView &hdr, GrbRows rows, void *schedule = nullptr, bool blocks_form = false,
-	                         const GrbStripes *stripes = nullptr);
+	                         Vulkan::ImageView &hdr, GrbRows rows, void *schedule = nullptr, const GrbStripes *stripes = nullptr);
 };
 
 // The "lighting" pass: reads albedo/normal/pbr/depth attachments + the cluster buffers, writes

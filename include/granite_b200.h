@@ -220,9 +220,9 @@ typedef struct GrbGBuffer
 int32_t grb_deferred_lighting(const GrbGBuffer *gbuffer, const GrbCamera *cam,
                               const GrbClusterParameters *params, const GrbClusterBuffers *buf,
                               const GrbImage *hdr, GrbRows rows, void *stream);
-/* Same pass as a plain grid of short-lived CTAs (no persistent CTAs, no schedule): the form for callers whose
- * other streams must get SMs while lighting runs, e.g. every rank of a row-sharded frame (granite_b200/csrc/
- * grb_lighting.cu).  Within the same parity bar; not bit-identical to the persistent form. */
+/* Same pass as a plain grid of short-lived CTAs (the non-persistent pairs kernel, no schedule): a CTA frees its SM
+ * when its block is done, where a persistent CTA holds it until the pass ends.  Within the same parity bar; not
+ * bit-identical to the persistent form. */
 int32_t grb_deferred_lighting_blocks(const GrbGBuffer *gbuffer, const GrbCamera *cam, const GrbClusterParameters *params,
                                      const GrbClusterBuffers *buf, const GrbImage *hdr, GrbRows rows, void *stream);
 /* Same pass with a caller-owned SCHEDULE buffer: grb_lighting_schedule_bytes(image height) bytes of
@@ -428,14 +428,13 @@ int32_t grb_fsr_sharpen(const GrbImage *color, const GrbImage *out, float sharpn
 int32_t grb_fxaa(const GrbImage *in, const GrbImage *out, GrbRows rows, void *stream);
 /* K13 taa_resolve.frag; renderer/post/temporal.cpp:226-265. history NULL on the first
  * frame (REPROJECTION_HISTORY=0). quality 0..2 = TAAQuality. mv: R16G16_SFLOAT.
- * out_color: B10G11R11_UFLOAT; out_history: R16G16B16A16_SFLOAT.  GRB_TAA_TILES=1 (the tile
- * kernel, quality 2 with history) applies to whole-frame calls, rows {0, 0}, only. */
+ * out_color: B10G11R11_UFLOAT; out_history: R16G16B16A16_SFLOAT. */
 int32_t grb_taa_resolve(const GrbImage *hdr, const GrbImage *depth, const GrbImage *mv,
                         const GrbImage *history, const float *reproj16, int32_t quality,
                         const GrbImage *out_color, const GrbImage *out_history, GrbRows rows, void *stream);
 /* grb_taa_resolve on the rows a rank of a row-sharded frame resolves, fused with the history exchange: a texel's
- * history read can land on any row, so every rank holds the whole history.  Colour (the values of the exact
- * grb_taa_resolve kernel; GRB_TAA_TILES does not apply) is written to out_color on [rows.y0, rows.y1).  The history
+ * history read can land on any row, so every rank holds the whole history.  Colour (the values of
+ * grb_taa_resolve) is written to out_color on [rows.y0, rows.y1).  The history
  * texel of each row of `own` (within rows) is stored into peer_images[r] for EVERY r, this rank's own slot
  * (peer_images[flag_index]) included; peer_images[r] is the base address, valid on this device, of rank r's history
  * image (cudaIpc-mapped peer memory), all with history_layout's size and pitch (history_layout->data is not used).

@@ -11,8 +11,7 @@ Cases:
   chain       the viewer's post chain on a fixed HDR image (the oracle's lit frame as emissive, no lights, sky
               everywhere) at 640x360 and 3840x2160, 3 frames: the frame, every pyramid level and average-luminance
   zrange      grb_cluster_build for 300 lights (25 % spots) at the 640x360 aspect: cluster-bitmask and cluster-range
-  lighting    grb_deferred_lighting on the 640x360 / 300 lights / 25 % spots case, then three grb_deferred_lighting_scheduled
-              launches on one schedule buffer: each frame, and the schedule after each launch
+  lighting    grb_deferred_lighting on the 640x360 / 300 lights / 25 % spots case
 """
 import os
 import sys
@@ -25,7 +24,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 SWITCHES = ("GRB_POST_EXACT", "GRB_POST_NO_TILES", "GRB_BLOOM_NO_FUSED_TAIL", "GRB_BLOOM_TAIL_CTAS", "GRB_ZRANGE_SCAN", "GRB_LIGHTING_V2",
-            "GRB_LIGHTING_1PX", "GRB_LIGHTING_ROW_BLOCKS")
+            "GRB_LIGHTING_1PX")
 LIGHTING_CASE = (640, 360, 300, 0.25)
 CHAIN_SIZES = ((640, 360), (3840, 2160))
 CHAIN_FRAMES = 3
@@ -141,18 +140,10 @@ def lighting(out_dir):
     from oracle import pyoracle as oracle
 
     oracle.build(ref=False)
-    scene, gb, dev, gcam = lighting_device_case(oracle)
-    res = {}
+    _, gb, dev, gcam = lighting_device_case(oracle)
     hdr = gb.emissive.clone()
     harness.deferred_lighting(gb, gcam, dev, hdr)
-    res["default"] = harness.to_host(hdr, np.uint32)
-    sched = harness.lighting_schedule(scene.depth.shape[0])
-    for i in range(3):
-        hdr = gb.emissive.clone()
-        harness.deferred_lighting(gb, gcam, dev, hdr, schedule=sched)
-        res[f"{i}/scheduled"] = harness.to_host(hdr, np.uint32)
-        res[f"{i}/schedule"] = harness.to_host(sched, np.uint32)
-    np.savez(os.path.join(out_dir, "lighting.npz"), **res)
+    np.savez(os.path.join(out_dir, "lighting.npz"), default=harness.to_host(hdr, np.uint32))
 
 
 def main():

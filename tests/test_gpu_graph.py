@@ -210,7 +210,7 @@ def test_taa_fxaa_chain(cuda, oracle, w, h, n):
         lum, d3_hist = f.lum, f.d3
         ldr = oracle.fxaa(f.ldr, True)
         got_res = v.download_image("HDR-resolved")
-        # TAA tile kernel: 1 code, or 2^-16 absolute for the nearly black pixels of a real frame (a code is 1e-6 there)
+        # 1 code, or 2^-16 absolute for the nearly black pixels of a real frame (a code is 1e-6 there)
         common.assert_r11g11b10_close(got_res, res_c, f"frame {i}: HDR-resolved", min_identical=0.97)
         d = common.rgba8_channel_diff(out, ldr)
         assert (d <= 1).mean() > 0.999, f"frame {i}"

@@ -10,8 +10,6 @@ GETENV = re.compile(r'getenv\(\s*"(GRB_[A-Z0-9_]+)"\s*\)')
 
 ALLOWED_UNTESTED = {
     "GRB_HOST_PROFILE": "prints host-side timings only; no computed value depends on it",
-    "GRB_SHARDED_BLOCKS": "selects grb_deferred_lighting_blocks for row-sharded frames; that form is tested on row bands in "
-                          "test_zo_gpu_lighting_forms.py, the switch itself needs a multi-rank run not written yet",
 }
 
 

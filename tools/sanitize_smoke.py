@@ -69,8 +69,6 @@ oc = torch.zeros((th, tw), dtype=torch.int32, device="cuda"); oh = harness.new_r
 mv_t = harness.to_dev(mv.reshape(th, tw, 2)).view(torch.int32).reshape(th, tw)
 for q in (0, 1, 2):
     harness.taa_resolve(harness.to_dev(thdr), harness.to_dev(depth), mv_t, harness.to_dev(thist), reproj, q, oc, oh)
-os.environ["GRB_TAA_TILES"] = "1"
-harness.taa_resolve(harness.to_dev(thdr), harness.to_dev(depth), mv_t, harness.to_dev(thist), reproj, 2, oc, oh)
 pq_out = torch.zeros((h, w), dtype=torch.int32, device="cuda")
 harness.pq10_encode(harness.to_dev(hdr), ldr, oracle.rec709_to_display_primaries(), 500.0, 400.0, 1000.0, pq_out)
 harness.pq10_encode(harness.to_dev(thdr), oc, oracle.rec709_to_display_primaries(), 500.0, 400.0, 1000.0, torch.zeros((th, tw), dtype=torch.int32, device="cuda"),
