@@ -27,6 +27,7 @@ UNITS = [
     ("grb_decal.cu", ["-fmad=false"]),
     ("grb_fog.cu", ["-fmad=false"]),
     ("grb_lighting.cu", []),
+    ("grb_gbuffer.cu", []),
 ]
 
 

@@ -84,6 +84,15 @@ class GrbGBuffer(C.Structure):
                 ("directional_color", C.c_float * 3), ("directional_direction", C.c_float * 3), ("emissive", GrbImage)]
 
 
+GBUFFER_PLANES = ("emissive", "albedo", "normal", "pbr", "depth", "mv")
+
+
+class GrbGBufferPlanes(C.Structure):
+    """A G-buffer as grb_gbuffer_copy_rows / grb_gbuffer_rows_to_peers take it: the planes in GBUFFER_PLANES order, a
+    NULL data pointer for an absent plane."""
+    _fields_ = [("plane", GrbImage * 6)]
+
+
 class GrbFogParameters(C.Structure):
     _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("depth", C.c_int32), ("dither_offset", C.c_int32),
                 ("slice_z_log2_scale", C.c_float), ("density_mod", C.c_float), ("in_scatter_strength", C.c_float)]
@@ -101,6 +110,7 @@ ENTRY_POINTS = [
     "grb_luminance", "grb_luminance_grid", "grb_luminance_finalize", "grb_bloom_tail", "grb_bloom_tail_ex", "grb_tonemap",
     "grb_pq10_encode", "grb_smaa_edge_detection", "grb_smaa_edge_detection_to_peers", "grb_smaa_blend_weights", "grb_smaa_neighborhood_blend", "grb_fsr_easu_constants", "grb_fsr_upscale", "grb_fsr_sharpen", "grb_fxaa", "grb_taa_resolve", "grb_taa_resolve_to_peers",
     "grb_present_rows_to_peer", "grb_deferred_lighting_stripes", "grb_hdr_rows_to_peers",
+    "grb_gbuffer_copy_rows", "grb_gbuffer_slot_layout", "grb_gbuffer_rows_to_peers",
 ]
 
 _lib = None
@@ -160,6 +170,9 @@ def lib() -> C.CDLL:
             "grb_deferred_lighting_stripes": [C.POINTER(GrbGBuffer), C.POINTER(GrbCamera), C.POINTER(GrbClusterParameters),
                                               C.POINTER(GrbClusterBuffers), C.POINTER(GrbLightShadows), IMG, GrbStripes, P, P],
             "grb_hdr_rows_to_peers": [IMG, P, P, C.POINTER(GrbRows), I, I, C.c_uint32, P, GrbStripes, P],
+            "grb_gbuffer_copy_rows": [C.POINTER(GrbGBufferPlanes), C.POINTER(GrbGBufferPlanes), C.POINTER(GrbRows), I, P],
+            "grb_gbuffer_slot_layout": [C.POINTER(GrbGBufferPlanes), P, C.POINTER(GrbGBufferPlanes), C.POINTER(C.c_uint64)],
+            "grb_gbuffer_rows_to_peers": [C.POINTER(GrbGBufferPlanes), P, P, C.POINTER(GrbRows), C.POINTER(C.c_int32), I, I, C.c_uint32, P, P],
         }
         for name, args in sig.items():
             fn = getattr(_lib, name)
@@ -197,6 +210,16 @@ def image(t, fmt: int) -> GrbImage:
     row = t.stride(0) * t.element_size()
     assert row == w * bpp, (row, w, bpp)
     return GrbImage(t.data_ptr(), w, h, row, fmt)
+
+
+def pitched_image(t, fmt: int) -> GrbImage:
+    """Wrap a CUDA tensor laid out (H, W[, C]) whose rows may be strided (a view into a wider allocation) as a GrbImage
+    of format `fmt`: the pitch is the tensor's row stride; every row's texels must be contiguous."""
+    assert t.is_cuda and t.dim() >= 2
+    h, w = int(t.shape[0]), int(t.shape[1])
+    bpp = TEXEL_BYTES[fmt]
+    assert t[0].is_contiguous() and t[0].numel() * t.element_size() == w * bpp, "a row's texels must be contiguous and of the format's size"
+    return GrbImage(t.data_ptr(), w, h, t.stride(0) * t.element_size(), fmt)
 
 
 def rows(r=None) -> GrbRows:

@@ -42,7 +42,7 @@ __device__ __forceinline__ void peer_publish(const PeerTargets &t)
 	__syncthreads();
 	if (threadIdx.x == 0 && threadIdx.y == 0)
 	{
-		const unsigned total = gridDim.x * gridDim.y;
+		const unsigned total = gridDim.x * gridDim.y * gridDim.z;
 		if (atomicAdd(t.ctas_done, 1u) == total - 1u)
 		{
 			*t.ctas_done = 0u;

@@ -371,6 +371,43 @@ def present_rows_to_peer(src_t, dst_t, flag_arrays, flag_index, epoch, counter_t
                "grb_present_rows_to_peer")
 
 
+def gbuffer_planes(**planes) -> capi.GrbGBufferPlanes:
+    """A GrbGBufferPlanes from keyword planes (capi.GBUFFER_PLANES names) given as (tensor, format): CUDA tensors laid
+    out (H, W[, C]) whose rows may be strided, the pitch being the row stride.  Planes not given are absent."""
+    g = capi.GrbGBufferPlanes()
+    for name, (t, fmt) in planes.items():
+        g.plane[capi.GBUFFER_PLANES.index(name)] = capi.pitched_image(t, fmt)
+    return g
+
+
+def gbuffer_copy_rows(src, dst, ranges):
+    """grb_gbuffer_copy_rows of the (y0, y1) `ranges` from the GrbGBufferPlanes src into dst on the current stream."""
+    rs = (capi.GrbRows * max(len(ranges), 1))(*[capi.GrbRows(int(a), int(b)) for a, b in ranges])
+    capi.check(capi.lib().grb_gbuffer_copy_rows(C.byref(src), C.byref(dst), rs, len(ranges), capi.stream_ptr()), "grb_gbuffer_copy_rows")
+
+
+def gbuffer_slot_layout(layout, base=None):
+    """grb_gbuffer_slot_layout: (the planes of a slot at device address `base`, the slot's bytes)."""
+    out, size = capi.GrbGBufferPlanes(), C.c_uint64()
+    capi.check(capi.lib().grb_gbuffer_slot_layout(C.byref(layout), None if base is None else C.c_void_p(base), C.byref(out), C.byref(size)),
+               "grb_gbuffer_slot_layout")
+    return out, size.value
+
+
+def gbuffer_rows_to_peers(src, slots, flag_arrays, rows_per_rank, flag_index, epoch, counter_t):
+    """grb_gbuffer_rows_to_peers with every rank's slot and flag array as tensors on this device: slots[q] a uint8
+    tensor of the slot's bytes (None for every rank: a flags-only publish), rows_per_rank[q] rank q's (y0, y1) list."""
+    n = len(flag_arrays)
+    flat = [r for lst in rows_per_rank for r in lst]
+    rs = (capi.GrbRows * max(len(flat), 1))(*[capi.GrbRows(int(a), int(b)) for a, b in flat])
+    counts = (C.c_int32 * n)(*[len(lst) for lst in rows_per_rank])
+    images = None if slots is None else (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_gbuffer_rows_to_peers(C.byref(src), images, flags, rs, counts, n, int(flag_index), int(epoch), _ptr(counter_t),
+                                                    capi.stream_ptr()),
+               "grb_gbuffer_rows_to_peers")
+
+
 def to_dev(a):
     return _dev(a)
 

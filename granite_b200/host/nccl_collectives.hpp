@@ -47,7 +47,7 @@ private:
 		std::vector<void *> opened;
 		uint32_t epoch = 0;
 	};
-	PeerState channels[(size_t)PeerChannel::HdrStripes + 1]; // [PeerChannel]
+	PeerState channels[(size_t)PeerChannel::GBuffer + 1]; // [PeerChannel]
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);
 };

@@ -84,6 +84,8 @@ public:
 		            // scene_viewer.cpp)
 		HdrStripes, // the HDR-main rows a rank lit in stripes that other ranks' lighting rows hold (the "lighting" and
 		            // "lighting-exchange" passes of scene_viewer.cpp)
+		GBuffer,    // the G-buffer rows each rank reads, pushed by the one rank that rasterised the whole frame into every
+		            // other rank's slot (the "gbuffer" pass of scene_viewer.cpp under grbh_viewer_set_gbuffer_source_rank)
 	};
 	struct PeerSlot
 	{

@@ -73,6 +73,9 @@ struct GrbhViewer
 		bool peer = false;
 		RenderGraphCollectives::PeerSlot slot;
 	} stripe_exchange;
+	// row-sharded frames fed from the one rank that rasterises the whole frame (-1: off;
+	// grbh_viewer_set_gbuffer_source_rank): its "gbuffer" pass pushes every rank's input rows into that rank's slot
+	int gbuffer_source = -1;
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
@@ -83,6 +86,10 @@ struct GrbhViewer
 	std::string output_name;
 	bool ui_layer_cleared = false;
 	const GrbhHostGBuffer *pending_upload = nullptr;
+	// this frame's G-buffer in device memory (grbh_viewer_render_frame_device), and how many passes still read it: the
+	// last of them records its `consumed` event
+	const GrbhDeviceGBuffer *pending_device = nullptr;
+	int device_reads_left = 0;
 	unsigned profiled_frames = 0;
 	std::map<std::string, std::pair<double, int>> timings;
 	std::vector<cudaEvent_t> pending_outputs; // one per async readback still in flight (oldest first)
@@ -137,7 +144,68 @@ struct GrbhViewer
 	}
 	// the G-buffer rows this rank must hold
 	std::vector<GrbRows> upload_ranges() const { return striped() ? stripe_plan().upload : std::vector<GrbRows>{ input_rows() }; }
+	// the same for rank q of the current bands
+	std::vector<GrbRows> upload_ranges_of(unsigned q) const
+	{
+		if (striped())
+			return compute_stripe_plan((unsigned)config.width, (unsigned)config.height, bands, q, uses_fxaa(), smaa_quality(), uses_taa(), lighting_stripes,
+			                           (unsigned)config.cluster_res[1])
+			    .upload;
+		return { compute_shard_plan((unsigned)config.width, (unsigned)config.height, bands, q, uses_fxaa(), smaa_quality(), uses_taa(), shard_upscale()).lighting };
+	}
 	bool sharded_presenting() const { return bands.size() > 1 && present_rank >= 0; }
+	bool fed_from_source() const { return bands.size() > 1 && gbuffer_source >= 0; }
+
+	// the G-buffer planes of the attachments (grb_gbuffer_copy_rows order), the G-buffer ones and / or motion vectors
+	GrbGBufferPlanes attachment_planes(bool gbuffer_planes, bool mv)
+	{
+		GrbGBufferPlanes a = {};
+		RenderTextureResource *res[GRB_GBUFFER_PLANES] = { res_emissive, res_albedo, res_normal, res_pbr, res_depth, res_mv };
+		for (int p = 0; p < GRB_GBUFFER_PLANES; p++)
+			if (res[p] && (p == 5 ? mv : gbuffer_planes))
+				a.plane[p] = graph.get_physical_texture_resource(*res[p]).as_grb();
+		return a;
+	}
+	static GrbGBufferPlanes caller_planes(const GrbhDeviceGBuffer &g, bool gbuffer_planes, bool mv)
+	{
+		GrbGBufferPlanes a = {};
+		if (gbuffer_planes)
+		{
+			a.plane[0] = g.emissive;
+			a.plane[1] = g.albedo;
+			a.plane[2] = g.normal;
+			a.plane[3] = g.pbr;
+			a.plane[4] = g.depth;
+		}
+		if (mv)
+			a.plane[5] = g.mv;
+		return a;
+	}
+	// a device G-buffer the viewer can read: every plane it needs, at the render size, in the attachment's format, with
+	// a pitch that holds a row and is a multiple of the texel.  "" when it is; no device needed.
+	std::string check_device_gbuffer(const GrbhDeviceGBuffer &g) const;
+	void wait_ready(cudaStream_t stream, const GrbhDeviceGBuffer &g)
+	{
+		if (g.ready)
+			Vulkan::cuda_ok(cudaStreamWaitEvent(stream, static_cast<cudaEvent_t>(g.ready), 0), "cudaStreamWaitEvent(ready)");
+	}
+	void record_consumed(cudaStream_t stream, const GrbhDeviceGBuffer &g)
+	{
+		if (g.consumed)
+			Vulkan::cuda_ok(cudaEventRecord(static_cast<cudaEvent_t>(g.consumed), stream), "cudaEventRecord(consumed)");
+	}
+	// the "gbuffer" / "mv" pass with a device G-buffer on one rank's own: the rank's rows of the planes the pass writes
+	void copy_device_rows(Vulkan::CommandBuffer &cmd, bool mv)
+	{
+		auto stream = reinterpret_cast<cudaStream_t>(cmd.get_stream());
+		wait_ready(stream, *pending_device);
+		const GrbGBufferPlanes src = caller_planes(*pending_device, !mv, mv), dst = attachment_planes(!mv, mv);
+		const std::vector<GrbRows> rows = upload_ranges();
+		cmd.check(grb_gbuffer_copy_rows(&src, &dst, rows.data(), (int32_t)rows.size(), cmd.get_stream_handle()), "grb_gbuffer_copy_rows");
+		if (--device_reads_left == 0)
+			record_consumed(stream, *pending_device);
+	}
+	void feed_from_source(Vulkan::CommandBuffer &cmd);
 
 	// the device-to-host copy of this rank's rows of the final image (the whole frame on the presenting rank), on the
 	// stream of the pass that produced it
@@ -228,7 +296,26 @@ void GrbhViewer::bake_render_graph()
 	res_normal = &gbuffer.add_color_output("normal", normal);
 	res_pbr = &gbuffer.add_color_output("pbr", pbr);
 	res_depth = &gbuffer.set_depth_stencil_output("depth-transient", depth);
+	// fed from one rank: the motion vectors come through the same channel, so this pass writes them too
+	res_mv = nullptr;
+	if (fed_from_source() && uses_taa())
+	{
+		AttachmentInfo mv;
+		mv.format = VK_FORMAT_R16G16_SFLOAT;
+		mv.size_x = mv.size_y = scene_scale();
+		res_mv = &gbuffer.add_color_output("mv-main", mv);
+	}
 	gbuffer.set_build_render_pass([this](Vulkan::CommandBuffer &cmd) {
+		if (fed_from_source())
+		{
+			feed_from_source(cmd);
+			return;
+		}
+		if (pending_device)
+		{
+			copy_device_rows(cmd, false);
+			return;
+		}
 		if (!pending_upload)
 			return; // inputs already resident from an earlier frame
 		upload_rows(cmd, res_emissive, pending_upload->emissive, config.render_target_fp16 ? 8 : 4);
@@ -326,8 +413,7 @@ void GrbhViewer::bake_render_graph()
 	case GRBH_AA_TAA_HIGH_PLUS_FXAA: before = PostAAType::TAA_High; break;
 	default: break;
 	}
-	res_mv = nullptr;
-	if (uses_taa())
+	if (uses_taa() && !fed_from_source())
 	{
 		// add_mv_pass: the motion-vector image is an input of this path
 		AttachmentInfo mv;
@@ -338,7 +424,9 @@ void GrbhViewer::bake_render_graph()
 		auto &mv_pass = graph.add_pass("mv", pipelined ? RENDER_GRAPH_QUEUE_ASYNC_COMPUTE_BIT : RENDER_GRAPH_QUEUE_GRAPHICS_BIT);
 		res_mv = &mv_pass.add_color_output("mv-main", mv);
 		mv_pass.set_build_render_pass([this](Vulkan::CommandBuffer &cmd) {
-			if (pending_upload)
+			if (pending_device)
+				copy_device_rows(cmd, true);
+			else if (pending_upload)
 				upload_rows(cmd, res_mv, pending_upload->mv, 4);
 		});
 	}
@@ -493,6 +581,134 @@ void GrbhViewer::bake_render_graph()
 	// keep feed-back buffers (average luminance) across re-bakes
 	graph.install_physical_buffers(std::move(physical_buffers));
 	baked = true;
+}
+
+std::string GrbhViewer::check_device_gbuffer(const GrbhDeviceGBuffer &g) const
+{
+	const int w = render_width(), h = render_height();
+	struct Plane
+	{
+		const char *name;
+		const GrbImage *image;
+		int32_t format, texel;
+		bool required;
+	};
+	const Plane planes[] = {
+		{ "emissive", &g.emissive, config.render_target_fp16 ? GRB_FORMAT_R16G16B16A16_SFLOAT : GRB_FORMAT_B10G11R11_UFLOAT_PACK32, config.render_target_fp16 ? 8 : 4,
+		  true },
+		{ "albedo", &g.albedo, GRB_FORMAT_R8G8B8A8_SRGB, 4, true },
+		{ "normal", &g.normal, GRB_FORMAT_A2B10G10R10_UNORM_PACK32, 4, true },
+		{ "pbr", &g.pbr, GRB_FORMAT_R8G8_UNORM, 2, true },
+		{ "depth", &g.depth, GRB_FORMAT_D32_SFLOAT, 4, true },
+		{ "mv", &g.mv, GRB_FORMAT_R16G16_SFLOAT, 4, uses_taa() },
+	};
+	for (const Plane &p : planes)
+	{
+		const GrbImage &im = *p.image;
+		const std::string name = std::string("the ") + p.name + " plane";
+		if (!p.required)
+			continue; // motion vectors without TAA: nothing reads them
+		if (!im.data)
+			return name + " is missing" + (std::string(p.name) == "mv" ? " (TAA reads the motion vectors)" : "");
+		if (im.width != w || im.height != h)
+			return name + " is " + std::to_string(im.width) + " x " + std::to_string(im.height) + "; the viewer renders at " + std::to_string(w) + " x " +
+			       std::to_string(h) + " (grbh_viewer_get_render_size)";
+		if (im.format != p.format)
+			return name + " has format " + std::to_string(im.format) + "; the attachment's is " + std::to_string(p.format);
+		if (im.row_pitch < w * p.texel || im.row_pitch % p.texel != 0)
+			return name + "'s row_pitch " + std::to_string(im.row_pitch) + " must be a multiple of its texel size (" + std::to_string(p.texel) +
+			       " bytes) and at least width x texel (" + std::to_string(w * p.texel) + ")";
+	}
+	return "";
+}
+
+// Feeding from the rank S that rasterised the whole frame (DESIGN.md section 5, "Feeding a sharded frame from one
+// rank").  Peer path: S waits for every rank's credit of the last epoch, pushes each rank q's input rows into q's slot
+// and copies its own; every other rank waits for S's flag, copies its rows out of its slot and raises its credit.
+// Without peer memory: S copies every rank's input rows into its own attachments, and per-plane NCCL broadcasts from
+// S write them into every rank's attachments in place.
+void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
+{
+	const unsigned S = (unsigned)gbuffer_source;
+	auto stream = reinterpret_cast<cudaStream_t>(cmd.get_stream());
+	void *handle = cmd.get_stream_handle();
+	const GrbGBufferPlanes attachments = attachment_planes(true, true);
+	const GrbhDeviceGBuffer *in = rank == S ? pending_device : nullptr;
+	if (rank == S && !in)
+		throw std::runtime_error("gbuffer: the source rank needs the whole frame's G-buffer every frame");
+	GrbGBufferPlanes src = {};
+	if (in)
+	{
+		wait_ready(stream, *in);
+		src = caller_planes(*in, true, uses_taa());
+	}
+	uint64_t bytes = 0;
+	if (!cmd.check(grb_gbuffer_slot_layout(&attachments, nullptr, nullptr, &bytes), "grb_gbuffer_slot_layout"))
+		return;
+	RenderGraphCollectives *coll = graph.get_collectives();
+	RenderGraphCollectives::PeerSlot slot;
+	if (coll->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::GBuffer, (size_t)bytes, slot))
+	{
+		if (rank == S)
+		{
+			// the credits: every rank copied the last epoch's rows out of its slot, and by stream order the epoch's before
+			cmd.check(grb_peer_wait(slot.flags[S], (int32_t)slot.count, slot.epoch - 1u, handle), "grb_peer_wait");
+			std::vector<GrbRows> rows;
+			std::vector<int32_t> counts;
+			for (unsigned q = 0; q < slot.count; q++)
+			{
+				const std::vector<GrbRows> r = q == S ? std::vector<GrbRows>{} : upload_ranges_of(q);
+				rows.insert(rows.end(), r.begin(), r.end());
+				counts.push_back((int32_t)r.size());
+			}
+			cmd.check(grb_gbuffer_rows_to_peers(&src, slot.images, slot.flags, rows.data(), counts.data(), (int32_t)slot.count, (int32_t)S, slot.epoch,
+			                                    slot.counter, handle),
+			          "grb_gbuffer_rows_to_peers");
+			const std::vector<GrbRows> own = upload_ranges();
+			cmd.check(grb_gbuffer_copy_rows(&src, &attachments, own.data(), (int32_t)own.size(), handle), "grb_gbuffer_copy_rows");
+			record_consumed(stream, *in);
+			return;
+		}
+		cmd.check(grb_peer_wait(slot.flags[rank] + S, 1, slot.epoch, handle), "grb_peer_wait");
+		GrbGBufferPlanes received = {};
+		cmd.check(grb_gbuffer_slot_layout(&attachments, slot.images[rank], &received, &bytes), "grb_gbuffer_slot_layout");
+		const std::vector<GrbRows> own = upload_ranges();
+		cmd.check(grb_gbuffer_copy_rows(&received, &attachments, own.data(), (int32_t)own.size(), handle), "grb_gbuffer_copy_rows");
+		// the credit: a flags-only publish once the rows are out of the slot
+		const std::vector<int32_t> none(slot.count, 0);
+		cmd.check(grb_gbuffer_rows_to_peers(&attachments, nullptr, slot.flags, nullptr, none.data(), (int32_t)slot.count, (int32_t)rank, slot.epoch,
+		                                    slot.counter, handle),
+		          "grb_gbuffer_rows_to_peers");
+		return;
+	}
+	// without peer memory: the union of every rank's input rows, broadcast from S
+	std::vector<GrbRows> all;
+	for (unsigned q = 0; q < bands.size(); q++)
+	{
+		const std::vector<GrbRows> r = upload_ranges_of(q);
+		all.insert(all.end(), r.begin(), r.end());
+	}
+	std::sort(all.begin(), all.end(), [](const GrbRows &a, const GrbRows &b) { return a.y0 < b.y0; });
+	std::vector<GrbRows> merged;
+	for (const GrbRows &r : all)
+	{
+		if (r.y1 <= r.y0)
+			continue;
+		if (!merged.empty() && r.y0 <= merged.back().y1)
+			merged.back().y1 = std::max(merged.back().y1, r.y1);
+		else
+			merged.push_back(r);
+	}
+	if (rank == S)
+	{
+		cmd.check(grb_gbuffer_copy_rows(&src, &attachments, merged.data(), (int32_t)merged.size(), handle), "grb_gbuffer_copy_rows");
+		record_consumed(stream, *in);
+	}
+	std::vector<std::vector<GrbRows>> lists(bands.size());
+	lists[S] = merged;
+	for (RenderTextureResource *res : { res_emissive, res_albedo, res_normal, res_pbr, res_depth, res_mv })
+		if (res && !coll->all_gather_row_lists(cmd, graph.get_physical_texture_resource(*res), lists))
+			throw std::runtime_error("gbuffer: the broadcast of the G-buffer rows from the source rank failed");
 }
 
 cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
@@ -864,6 +1080,9 @@ extern "C" int32_t grbh_viewer_set_row_shards(GrbhViewer *v, const GrbRows *band
 	if (v->present_rank >= std::max(count, 1))
 		return fail("grbh_viewer_set_row_shards: the presenting rank " + std::to_string(v->present_rank) + " would have no band among " +
 		            std::to_string(count) + " (call grbh_viewer_set_present_rank first)");
+	if (v->gbuffer_source >= std::max(count, 1))
+		return fail("grbh_viewer_set_row_shards: the G-buffer source rank " + std::to_string(v->gbuffer_source) + " would have no band among " +
+		            std::to_string(count) + " (call grbh_viewer_set_gbuffer_source_rank first)");
 	v->bands.assign(bands, bands + count);
 	v->rank = (unsigned)rank;
 	v->baked = false;
@@ -882,6 +1101,35 @@ extern "C" int32_t grbh_viewer_set_present_rank(GrbhViewer *v, int32_t rank)
 	v->present_rank = rank;
 	v->baked = false;
 	return 0;
+}
+
+extern "C" int32_t grbh_viewer_set_gbuffer_source_rank(GrbhViewer *v, int32_t rank)
+{
+	if (!v)
+		return fail("null viewer");
+	const int32_t count = std::max((int32_t)v->bands.size(), 1); // an unsharded viewer is one band
+	if (rank < -1 || rank >= count)
+		return fail("grbh_viewer_set_gbuffer_source_rank: rank must be -1 (off) or within [0, " + std::to_string(count) +
+		            ") (the bands of the last grbh_viewer_set_row_shards)");
+	if (rank >= 0 && v->config.pipelined_io)
+		return fail("grbh_viewer_set_gbuffer_source_rank: not with pipelined_io (the G-buffer channel already keeps two slots in flight)");
+	v->gbuffer_source = rank;
+	v->baked = false;
+	return 0;
+}
+
+extern "C" int32_t grbh_viewer_get_input_rows(GrbhViewer *v, GrbRows *out, int32_t capacity)
+{
+	if (!v || capacity < 0)
+		return fail("grbh_viewer_get_input_rows: bad arguments");
+	GRBH_TRY
+	const std::vector<GrbRows> rows = v->upload_ranges();
+	if (out && (int64_t)rows.size() > capacity)
+		return fail("grbh_viewer_get_input_rows: the rank reads " + std::to_string(rows.size()) + " row ranges, capacity is " + std::to_string(capacity));
+	if (out)
+		std::copy(rows.begin(), rows.end(), out);
+	return (int32_t)rows.size();
+	GRBH_CATCH
 }
 
 extern "C" int32_t grbh_viewer_set_lighting_stripes(GrbhViewer *v, int32_t stripe_rows)
@@ -1068,6 +1316,9 @@ extern "C" int32_t grbh_viewer_bake(GrbhViewer *v)
 
 extern "C" int32_t grbh_viewer_render_frame(GrbhViewer *v, const GrbhHostGBuffer *host, double frame_time)
 {
+	if (v && v->fed_from_source())
+		return fail("grbh_viewer_render_frame: the frame is fed from the G-buffer source rank (grbh_viewer_set_gbuffer_source_rank); every rank calls "
+		            "grbh_viewer_render_frame_device");
 	if (!v || !v->baked)
 		return fail("grbh_viewer_render_frame: viewer not baked");
 	if (v->config.pipelined_io && !host)
@@ -1079,6 +1330,57 @@ extern "C" int32_t grbh_viewer_render_frame(GrbhViewer *v, const GrbhHostGBuffer
 	GRBH_TRY
 	cudaSetDevice(v->device->get_device_index());
 	v->render_frame(host, frame_time);
+	v->bands_moved = false;
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_render_frame_device(GrbhViewer *v, const GrbhDeviceGBuffer *gbuffer, double frame_time)
+{
+	const char *fn = "grbh_viewer_render_frame_device: ";
+	if (!v)
+		return fail(std::string(fn) + "null viewer");
+	if (v->fed_from_source())
+	{
+		const bool source = v->rank == (unsigned)v->gbuffer_source;
+		if (source && !gbuffer)
+			return fail(std::string(fn) + "this rank is the G-buffer source rank (grbh_viewer_set_gbuffer_source_rank): it passes the whole frame's G-buffer every frame");
+		if (!source && gbuffer)
+			return fail(std::string(fn) + "the frame is fed from G-buffer source rank " + std::to_string(v->gbuffer_source) +
+			            " (grbh_viewer_set_gbuffer_source_rank); every other rank passes NULL");
+	}
+	if (gbuffer)
+	{
+		const std::string bad = v->check_device_gbuffer(*gbuffer);
+		if (!bad.empty())
+			return fail(fn + bad);
+	}
+	if (!v->device)
+		return fail(std::string(fn) + "host-only viewer (cuda_device < 0) has no device to read a G-buffer on");
+	if (!v->baked)
+		return fail(std::string(fn) + "viewer not baked");
+	if (!v->fed_from_source())
+	{
+		if (v->config.pipelined_io && !gbuffer)
+			return fail(std::string(fn) + "pipelined_io viewers need a G-buffer every frame");
+		if (v->bands_moved && !gbuffer)
+			return fail(std::string(fn) + "the bands moved (grbh_viewer_move_row_shards) since the last frame and the resident G-buffer holds the old rows; "
+			                              "this frame must bring a G-buffer");
+	}
+	GRBH_TRY
+	cudaSetDevice(v->device->get_device_index());
+	v->pending_device = gbuffer;
+	v->device_reads_left = v->uses_taa() ? 2 : 1;
+	try
+	{
+		v->render_frame(nullptr, frame_time);
+	}
+	catch (...)
+	{
+		v->pending_device = nullptr;
+		throw;
+	}
+	v->pending_device = nullptr;
 	v->bands_moved = false;
 	return 0;
 	GRBH_CATCH

@@ -37,6 +37,11 @@ class GrbhHostGBuffer(C.Structure):
                 ("emissive", C.c_void_p), ("mv", C.c_void_p)]
 
 
+class GrbhDeviceGBuffer(C.Structure):
+    _fields_ = [("emissive", capi.GrbImage), ("albedo", capi.GrbImage), ("normal", capi.GrbImage), ("pbr", capi.GrbImage),
+                ("depth", capi.GrbImage), ("mv", capi.GrbImage), ("ready", C.c_void_p), ("consumed", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -53,6 +58,8 @@ def lib() -> C.CDLL:
         _lib.grbh_viewer_destroy.restype = None
         _lib.grbh_viewer_destroy.argtypes = [C.c_void_p]
         _lib.grbh_viewer_render_frame.argtypes = [C.c_void_p, C.POINTER(GrbhHostGBuffer), C.c_double]
+        _lib.grbh_viewer_render_frame_device.argtypes = [C.c_void_p, C.POINTER(GrbhDeviceGBuffer), C.c_double]
+        _lib.grbh_viewer_get_input_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         _lib.grbh_viewer_set_exposure.argtypes = [C.c_void_p, C.c_float]
     return _lib
 
@@ -407,6 +414,20 @@ class Viewer:
         frame.  Every rank sets the same value, before bake."""
         _check(lib().grbh_viewer_set_present_rank(self._h, int(rank)), "grbh_viewer_set_present_rank")
 
+    def set_gbuffer_source_rank(self, rank):
+        """Feed row-sharded frames from `rank`, which rasterises the whole frame (-1: off): every rank then calls
+        render_frame_device every frame, that rank with the whole G-buffer and every other rank with None.  Every rank
+        sets the same value, before bake; not with pipelined_io (grbh_viewer_set_gbuffer_source_rank)."""
+        _check(lib().grbh_viewer_set_gbuffer_source_rank(self._h, int(rank)), "grbh_viewer_set_gbuffer_source_rank")
+
+    def input_rows(self):
+        """The (y0, y1) row ranges of the render-size G-buffer this rank reads: the rows a sort-first rasteriser on this
+        rank must produce, and the only rows of a device G-buffer that must be valid (grbh_viewer_get_input_rows)."""
+        n = _check(lib().grbh_viewer_get_input_rows(self._h, None, 0), "grbh_viewer_get_input_rows")
+        out = (capi.GrbRows * max(n, 1))()
+        n = _check(lib().grbh_viewer_get_input_rows(self._h, out, n), "grbh_viewer_get_input_rows")
+        return [(out[i].y0, out[i].y1) for i in range(n)]
+
     def move_row_shards(self, bands):
         """Move the band cuts of a baked row-sharded viewer from the next frame on, without a re-bake: the TAA history,
         bloom feedback and every attachment carry over.  Same band count; the bands tile [0, height).  The next
@@ -430,6 +451,31 @@ class Viewer:
     def render_frame(self, host_gbuffer: GrbhHostGBuffer | None, frame_time=1.0 / 60.0):
         arg = C.byref(host_gbuffer) if host_gbuffer is not None else None
         _check(lib().grbh_viewer_render_frame(self._h, arg, C.c_double(frame_time)), "grbh_viewer_render_frame")
+
+    def device_gbuffer(self, albedo, normal, pbr, depth, emissive, mv=None) -> GrbhDeviceGBuffer:
+        """A G-buffer in device memory from torch CUDA tensors on the viewer's device, (H, W[, C]) at render_size(), in
+        host_gbuffer's layouts (albedo / normal / depth / mv: 4 bytes per texel, pbr: 2, emissive: 4, or (H, W, 4)
+        16-bit with render_target_fp16).  A tensor's rows may be strided (a view of a padded image): each pitch is the
+        tensor's row stride.  The tensors must stay alive, and unwritten, until the frame's `consumed` event."""
+        def img(t, fmt):
+            return capi.GrbImage() if t is None else capi.pitched_image(t, fmt)
+        em = capi.FORMAT_R16G16B16A16_SFLOAT if emissive is not None and emissive.dim() == 3 else capi.FORMAT_B10G11R11_UFLOAT
+        return GrbhDeviceGBuffer(img(emissive, em), img(albedo, capi.FORMAT_R8G8B8A8_SRGB), img(normal, capi.FORMAT_A2B10G10R10_UNORM),
+                                 img(pbr, capi.FORMAT_R8G8_UNORM), img(depth, capi.FORMAT_D32_SFLOAT), img(mv, capi.FORMAT_R16G16_SFLOAT))
+
+    def render_frame_device(self, gb: GrbhDeviceGBuffer | None, ready=None, consumed=None, frame_time=1.0 / 60.0):
+        """The frame render_frame renders from a host G-buffer with the same bytes, from gb in device memory (None:
+        the resident G-buffer, or a non-source rank under set_gbuffer_source_rank).  ready: a torch.cuda.Event the copy
+        waits on; consumed: a torch.cuda.Event the viewer records after its last read of gb's memory."""
+        arg = None
+        if gb is not None:
+            arg = GrbhDeviceGBuffer.from_buffer_copy(gb)
+            arg.ready = None if ready is None else (ready.cuda_event or None)
+            if consumed is not None and not consumed.cuda_event:
+                consumed.record()  # torch creates the CUDA event on its first record
+            arg.consumed = None if consumed is None else consumed.cuda_event
+            arg = C.byref(arg)
+        _check(lib().grbh_viewer_render_frame_device(self._h, arg, C.c_double(frame_time)), "grbh_viewer_render_frame_device")
 
     def read_output(self, dst):
         """dst: full-frame uint32 buffer (numpy array or pinned torch tensor). Returns the (y0, y1) band written."""

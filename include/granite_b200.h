@@ -477,6 +477,44 @@ int32_t grb_hdr_rows_to_peers(const GrbImage *hdr, void *const *peer_images, uin
                               int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, GrbStripes stripes,
                               void *stream);
 
+/* ---- G-buffers in device memory ----
+ * The G-buffer the lighting pass reads, as up to six planes in this order: emissive (B10G11R11_UFLOAT, or
+ * R16G16B16A16_SFLOAT with renderTargetFp16), albedo (R8G8B8A8_SRGB), normal (A2B10G10R10_UNORM_PACK32), pbr
+ * (R8G8_UNORM), depth (D32_SFLOAT), mv (R16G16_SFLOAT).  A plane whose data is NULL is absent.  Every present plane has
+ * one size, a row_pitch that is a multiple of its texel size and at least width x texel (padded images and strided
+ * tensors are fine), and a base aligned to its texel size.  Both copies below are byte copies, so they are exact. */
+#define GRB_GBUFFER_PLANES 6
+typedef struct GrbGBufferPlanes
+{
+	GrbImage plane[GRB_GBUFFER_PLANES]; /* emissive, albedo, normal, pbr, depth, mv */
+} GrbGBufferPlanes;
+/* Copies rows[0..range_count) (ranges of the image, empty allowed) of every present plane of src into dst, in one
+ * launch per 128 ranges.  Only the listed rows are written, and of each only width x texel bytes (a pitch's padding is
+ * left alone).  16-byte loads and stores where the plane's pitches and bases allow it, whole texels otherwise.
+ * GRB_ERR_INVALID_ARGUMENT: a null pointer, a negative count, a plane that breaks the rules above, src and dst with
+ * different planes present, sizes or formats, a dst plane that is its src plane, a range outside the image (checked
+ * before any CUDA call; nothing is written).  No reference equivalent: in the reference the G-buffer pass rasterises
+ * into the attachments the lighting pass reads. */
+int32_t grb_gbuffer_copy_rows(const GrbGBufferPlanes *src, const GrbGBufferPlanes *dst, const GrbRows *rows, int32_t range_count,
+                              void *stream);
+/* The G-buffer slot of a row-sharded frame's "gbuffer" channel: the present planes of `layout` (size and formats; its
+ * data pointers only mark presence) packed one after another from `base`, each with the pitch width x texel and from
+ * a multiple of 256 bytes.  *bytes receives the slot's size; out (may be NULL) the planes at `base` (NULL data when
+ * base is NULL).  GRB_ERR_INVALID_ARGUMENT as grb_gbuffer_copy_rows for the layout. */
+int32_t grb_gbuffer_slot_layout(const GrbGBufferPlanes *layout, void *base, GrbGBufferPlanes *out, uint64_t *bytes);
+/* Feeding a row-sharded frame from the one rank that rasterised it: copies rank q's ranges (range_counts[q] of them,
+ * the lists of rows one after another, empty ranges allowed) of every present plane of src into peer_slots[q], the
+ * base address, valid on this device, of rank q's slot (cudaIpc-mapped peer memory; the layout of
+ * grb_gbuffer_slot_layout for src's planes), rows at their place.  Then flags[flag_index] = epoch is release-stored
+ * into the flag array of EVERY rank.  peer_slots may be NULL when no range is listed: a flags-only publish (the credit a
+ * receiving rank raises once it has copied its rows out of its slot).  scratch_counter: one zero-initialised uint32 in
+ * local device memory.  GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index
+ * outside 0..peer_count-1, a negative count, src's planes as for grb_gbuffer_copy_rows, a range outside the image
+ * (checked before any CUDA call; nothing is written).  No reference equivalent (the reference never splits a frame). */
+int32_t grb_gbuffer_rows_to_peers(const GrbGBufferPlanes *src, void *const *peer_slots, uint32_t *const *peer_flags, const GrbRows *rows,
+                                  const int32_t *range_counts, int32_t peer_count, int32_t flag_index, uint32_t epoch,
+                                  uint32_t *scratch_counter, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,7 +5,8 @@
  * setup_fxaa_postprocess) the way SceneViewerApplication does in the reference
  * (application/scene_viewer_application.cpp:876-991 add_main_pass_deferred, :1167-1318
  * bake_render_graph, :1540-1611 render_frame).  The G-buffer, which the reference rasterises,
- * is an INPUT here: it is uploaded from host memory by a "gbuffer" pass at the head of the graph.
+ * is an INPUT here: a "gbuffer" pass at the head of the graph uploads it from host memory
+ * (grbh_viewer_render_frame) or copies it from device memory (grbh_viewer_render_frame_device).
  *
  * This is what bench.py's end-to-end measurement and the graph-level tests call.  All
  * functions return 0 on success, negative on failure (grbh_last_error()).
@@ -97,6 +98,21 @@ typedef struct GrbhHostGBuffer
 	const uint32_t *mv; /* R16G16_SFLOAT */
 } GrbhHostGBuffer;
 
+/* A G-buffer in device memory on the viewer's device, at the render size (grbh_viewer_get_render_size), each plane in
+ * its attachment's format: emissive B10G11R11_UFLOAT (R16G16B16A16_SFLOAT with render_target_fp16), albedo
+ * R8G8B8A8_SRGB, normal A2B10G10R10_UNORM_PACK32, pbr R8G8_UNORM, depth D32_SFLOAT, mv R16G16_SFLOAT (needed under TAA
+ * only).  row_pitch: any multiple of the texel size of at least width x texel (padded images, strided tensors).  Only
+ * the rows of grbh_viewer_get_input_rows are read.
+ * ready: an event the "gbuffer" pass waits on before it reads, or NULL (the caller orders its writes before the frame).
+ * consumed: a caller-created event, or NULL; the viewer records it right after its last read of the caller's memory,
+ * so the caller may overwrite its buffers once it has completed. */
+typedef struct GrbhDeviceGBuffer
+{
+	GrbImage emissive, albedo, normal, pbr, depth, mv;
+	void *ready;    /* cudaEvent_t */
+	void *consumed; /* cudaEvent_t */
+} GrbhDeviceGBuffer;
+
 const char *grbh_last_error(void);
 
 int32_t grbh_viewer_create(const GrbhViewerConfig *config, GrbhViewer **out);
@@ -164,6 +180,20 @@ int32_t grbh_viewer_set_lighting_stripes(GrbhViewer *viewer, int32_t stripe_rows
  * (the checks give every rank the same answer for the same input).  Ranks that disagree on the layout run mismatched
  * exchanges. */
 int32_t grbh_viewer_move_row_shards(GrbhViewer *viewer, const GrbRows *bands, int32_t count);
+/* Row-sharded frames fed from the one rank that rasterises the whole frame: rank -1 = off (the default), otherwise
+ * within [0, band count) of the last grbh_viewer_set_row_shards (an unsharded viewer counts as one band and changes
+ * nothing).  Every rank then calls grbh_viewer_render_frame_device every frame, that rank with the whole frame's
+ * G-buffer and every other rank with NULL; grbh_viewer_render_frame is refused.  The source rank's "gbuffer" pass pushes
+ * each rank's input rows (grbh_viewer_get_input_rows of that rank, from the current bands) into that rank's slot of a
+ * double-buffered peer channel and each rank copies them into its attachments (DESIGN.md section 5, "Feeding a sharded
+ * frame from one rank"); without peer memory the rows go out in NCCL broadcasts.  Call before bake, with the same value
+ * on every rank.  Refused with pipelined_io. */
+int32_t grbh_viewer_set_gbuffer_source_rank(GrbhViewer *viewer, int32_t rank);
+/* The row ranges of the render-size G-buffer this rank reads: its lighting rows (grbh_shard_plan*), or the upload list
+ * of grbh_shard_plan_stripes under lighting in stripes; {0, render height} unsharded.  These are the rows a sort-first
+ * rasteriser on this rank must produce: a device G-buffer needs only these rows to be valid.  Returns the count;
+ * out = NULL only counts.  Pure host math of the current bands. */
+int32_t grbh_viewer_get_input_rows(GrbhViewer *viewer, GrbRows *out, int32_t capacity);
 
 /* Work estimate of the lighting pass per group of 4 rows of the render-size image (the backbuffer without FSR 1) for
  * the frame last rendered: grb_lighting_row_cost() on the viewer's depth image and light cluster, copied to the host.
@@ -220,6 +250,14 @@ int32_t grbh_viewer_bake(GrbhViewer *viewer);
 /* One frame: (optionally) upload the host G-buffer rows, refresh the clusterer, record every
  * pass on the stream.  Asynchronous; ordering with later calls is stream order. */
 int32_t grbh_viewer_render_frame(GrbhViewer *viewer, const GrbhHostGBuffer *host_gbuffer, double frame_time);
+/* The same frame from a G-buffer in device memory: bit for bit the frame grbh_viewer_render_frame renders from a host
+ * G-buffer holding the same bytes.  The "gbuffer" and "mv" passes copy this rank's input rows into the attachments
+ * (grb_gbuffer_copy_rows; on the side stream into the alternating images with pipelined_io).  NULL: light the resident
+ * G-buffer again, as grbh_viewer_render_frame(NULL) (refused with pipelined_io and on the first frame after
+ * grbh_viewer_move_row_shards).  Refused: a missing plane (mv under TAA), a plane not at the render size or not in its
+ * attachment's format, a pitch too small or not a multiple of the texel size, a host-only viewer; and under
+ * grbh_viewer_set_gbuffer_source_rank a NULL G-buffer on the source rank or a G-buffer on any other. */
+int32_t grbh_viewer_render_frame_device(GrbhViewer *viewer, const GrbhDeviceGBuffer *gbuffer, double frame_time);
 /* Copies this rank's rows of the final image (R8G8B8A8) to host memory laid out as the full
  * frame (row pitch = width*4) and waits for it. rows_out receives the band (the whole frame on
  * the presenting rank, grbh_viewer_set_present_rank). */
