@@ -91,7 +91,12 @@ GRB_SHADOW_DEV float shadow_sample_2d_wide(const uint16_t *map, int res, float c
 	const float ix = __fsub_rn(__fmul_rn(u, fres), 1.5f), iy = __fsub_rn(__fmul_rn(v, fres), 1.5f);
 	const float flx = floorf(ix), fly = floorf(iy);
 	const float fx = __fsub_rn(ix, flx), fy = __fsub_rn(iy, fly);
-	const ShadowBilin q = shadow_bilin(__fdiv_rn(flx, fres), __fdiv_rn(fly, fres), res); // origin of the first gather's footprint
+	// origin of the first gather's footprint: floor(flx / res * res - 0.5) = flx - 1.  Not clamped to the map: each texel
+	// of the 6 x 6 window clamps to the edge on its own, as the gathers' clamp-to-edge does, so near the low edge the
+	// window repeats texel 0 as often as it reaches past it.  Beyond 8 texels outside every texel clamps to the same
+	// edge, so the bound only keeps the int conversion defined; NaN coordinates give the origin -1.
+	const ShadowBilin q = { (int)(flx == flx ? fminf(fmaxf(flx, -8.0f), fres + 8.0f) : 0.0f) - 1,
+		                    (int)(fly == fly ? fminf(fmaxf(fly, -8.0f), fres + 8.0f) : 0.0f) - 1, 0.0f, 0.0f };
 	float H[6], V[6];
 	const float off[6] = { 2.0f, 1.0f, 0.0f, -1.0f, -2.0f, -3.0f };
 #pragma unroll

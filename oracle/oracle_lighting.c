@@ -141,8 +141,13 @@ float orc_shadow_sample_2d_wide(const uint16_t *map, int res, float clip_x, floa
 	float ix = u * fres - 1.5f, iy = v * fres - 1.5f;
 	float flx = floorf(ix), fly = floorf(iy);
 	const float fx = ix - flx, fy = iy - fly;
-	/* footprint origin of textureGather at floored / res: floor(floored / res * res - 0.5) = floored - 1 */
-	bilin_t b = bilin_setup(flx / fres, fly / fres, res, res);
+	/* footprint origin of textureGather at floored / res: floor(floored / res * res - 0.5) = floored - 1.  Each texel of
+	 * the window clamps to the edge on its own (the gathers' clamp to edge), so the origin itself is not clamped to the
+	 * map; 8 texels outside, every texel already clamps to the same edge, so the bound only keeps the int conversion
+	 * defined.  NaN coordinates: origin -1. */
+	bilin_t b;
+	b.x0 = (int)(flx == flx ? f_clamp(flx, -8.0f, fres + 8.0f) : 0.0f) - 1;
+	b.y0 = (int)(fly == fly ? f_clamp(fly, -8.0f, fres + 8.0f) : 0.0f) - 1;
 	float H[6], V[6];
 	const float off[6] = { 2.0f, 1.0f, 0.0f, -1.0f, -2.0f, -3.0f };
 	for (int i = 0; i < 6; i++)

@@ -179,14 +179,14 @@ def assert_r11g11b10_close(got, ref, what="", abs_floor=2.0 ** -16, min_identica
     return ident
 
 
-def make_shadow_maps(prep, resolution, seed=0x5AD0, skip_every=7):
-    """Synthetic D16 shadow maps, one per light of prep (cluster order): blocks of 4 x 4 texels holding depths spread
+def make_shadow_maps(prep, resolution, seed=0x5AD0, skip_every=7, block=4):
+    """Synthetic D16 shadow maps, one per light of prep (cluster order): blocks of block x block texels holding depths spread
     over the range the receivers' reference depths fall in (reverse-Z with near = 0.5 % of the light's range: a
     receiver at 10 % .. 100 % of the range compares 0.045 .. 0 against the map), so footprints come out lit, shadowed
     and partially lit.  Every skip_every-th light has no map (casts no shadow).  Spot: (res, res); point: (6, res, res)."""
     rng = np.random.default_rng(seed + prep.n)
     maps = []
-    blocks = (resolution + 3) // 4
+    blocks = (resolution + block - 1) // block
     for i in range(prep.n):
         if skip_every and i % skip_every == skip_every - 1:
             maps.append(None)
@@ -195,7 +195,7 @@ def make_shadow_maps(prep, resolution, seed=0x5AD0, skip_every=7):
         faces = 6 if is_point else 1
         coarse = rng.integers(0, 3000, (faces, blocks, blocks)).astype(np.uint16)
         coarse[rng.random(coarse.shape) < 0.3] = 0  # open sky: everything in front of the far plane is lit
-        m = np.repeat(np.repeat(coarse, 4, axis=1), 4, axis=2)[:, :resolution, :resolution]
+        m = np.repeat(np.repeat(coarse, block, axis=1), block, axis=2)[:, :resolution, :resolution]
         maps.append(np.ascontiguousarray(m if is_point else m[0]))
     return maps
 

@@ -41,14 +41,14 @@ def _check_stripes(whole, run_stripes, sentinel, h):
         assert (got[~inside] == sentinel).all(), f"stripes {s}: a row outside the set was written"
 
 
-@pytest.mark.parametrize("form", ["persistent", "rgba16f", "shadowed"])
+@pytest.mark.parametrize("form", ["persistent", "rgba16f", "shadowed", "shadowed-rgba16f"])
 def test_stripes_equal_whole_image_lighting(cuda, oracle, form):
     import torch
 
     from granite_b200 import capi, harness
     from tests.test_gpu_parity import _cluster
 
-    if form == "shadowed":
+    if form.startswith("shadowed"):
         from tests.test_oracle_ref_light_shadows import shadow_case
         from tests.test_zy_gpu_shadows import _device_shadows
 
@@ -62,7 +62,7 @@ def test_stripes_equal_whole_image_lighting(cuda, oracle, form):
         shadows = None
     dev, gcam = _cluster(cuda, oracle, cam, prep)
     gb = harness.GBufferDevice(scene)
-    if form == "rgba16f":
+    if form.endswith("rgba16f"):
         em = harness.to_dev(common.random_hdr_f16(np.random.default_rng(3), w, h, scale=0.02, hot=0.001))
         emissive_img = capi.image(em, capi.FORMAT_R16G16B16A16_SFLOAT)
         new_hdr = lambda: torch.full((h, w, 4), 0x2AB5, dtype=torch.int16, device="cuda")

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests import common
+from tests import lighting_ref64 as R
 
 pytestmark = pytest.mark.gpu
 
@@ -41,6 +42,8 @@ def test_cuda_lighting_into_fp16_hdr(cuda, oracle, w, h, n, spots):
     exact = float((d.max(-1) == 0).mean())
     print(f"fp16 lighting: max code diff {int(d.max())}, exact pixels {exact:.4f}")
     assert d.max() <= 2 and (d <= 1).mean() > 0.9999 and exact > 0.8
+    share = R.assert_meets_bar(got, R.reference(oracle, scene, cam, prep, clus, emissive=em16, fmt=R.RGBA16F), f"fp16 {w}x{h}")
+    print(f"fp16 lighting: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
     # row bands are bit-invariant
     cut = (h // 3) & ~3
     hdr2 = harness.to_dev(em16)
@@ -105,6 +108,7 @@ def test_viewer_frame_with_fp16_render_target(cuda, oracle):
     cam, prep = common.build_case_for_viewer(oracle, v, scene, lights)
     clus = oracle.cluster_build(cam, prep)
     hdr_ref = oracle.deferred_lighting_fp16(scene, cam, prep, clus, em16)
+    ref64 = R.reference(oracle, scene, cam, prep, clus, emissive=em16, fmt=R.RGBA16F)
     lum, d3 = np.zeros(3, np.float32), None
     out = np.zeros((h, w), np.uint32)
     for i in range(2):
@@ -115,6 +119,8 @@ def test_viewer_frame_with_fp16_render_target(cuda, oracle):
         hdr_dev = v.download_image("HDR-main")
         d = _f16_code_diff(hdr_dev[..., :3], hdr_ref[..., :3])
         assert d.max() <= 2 and (d.max(-1) == 0).mean() > 0.8
+        share = R.assert_meets_bar(hdr_dev, ref64, f"viewer fp16 frame {i}")
+        print(f"viewer fp16 frame {i}: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
         # the post chain is checked on the HDR image the device itself produced
         f = oracle.hdr_chain(hdr_dev, lum, d3)
         lum, d3 = f.lum, f.d3

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 
 from tests import common
+from tests import lighting_ref64 as R
 from tests.test_oracle_ref_light_shadows import shadow_case
 
 pytestmark = pytest.mark.gpu
@@ -58,6 +59,11 @@ def test_cuda_shadowed_lighting_vs_oracle(cuda, oracle, w, h, n, spots, res):
     sky = scene.depth == 0
     assert np.array_equal(got[sky], scene.emissive[sky]), "sky pixels must keep the attachment value"
     _compare(got, ref, 0.97)
+    # 1080p: the float64 reference of the whole frame holds ~6 M pairs, so it is held to the bar on 128 rows across
+    # the middle of the frame, where the lights crowd
+    band = (h // 2 - 64, h // 2 + 64) if h > 720 else None
+    share = R.assert_meets_bar(got, R.reference(oracle, scene, cam, prep, clus, shadows=(transforms, maps, res), rows=band), "shadowed")
+    print(f"shadowed lighting: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
     assert (ref != oracle.deferred_lighting(scene, cam, prep, clus)).mean() > 0.001, "the case must actually shadow pixels"
     # no maps at all == the unshadowed pass of the same kernel family
     none = _gpu_shadowed(cuda, oracle, scene, cam, prep, transforms, [None] * prep.n, res)
@@ -73,7 +79,23 @@ def test_cuda_wide_pcf_vs_oracle(cuda, oracle):
     """SHADOW_MAP_PCF_KERNEL_WIDE: the 6 x 6 kernel of the spot lights (its exp2 is CUDA's on hardware: lighting bar)."""
     scene, cam, prep, clus, transforms, maps = shadow_case(oracle, 320, 180, 300, 0.6, 64)
     ref = oracle.deferred_lighting_shadowed(scene, cam, prep, clus, transforms, maps, 64, pcf_wide=True)
-    _compare(_gpu_shadowed(cuda, oracle, scene, cam, prep, transforms, maps, 64, pcf_wide=True), ref, 0.97)
+    got = _gpu_shadowed(cuda, oracle, scene, cam, prep, transforms, maps, 64, pcf_wide=True)
+    _compare(got, ref, 0.97)
+    share = R.assert_meets_bar(got, R.reference(oracle, scene, cam, prep, clus, shadows=(transforms, maps, 64, True)), "wide PCF")
+    print(f"wide PCF: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
+
+
+@pytest.mark.parametrize("case", ["spot-edge-narrow-res8", "spot-edge-wide-res8"])
+def test_cuda_spot_edges_meet_the_float64_bar(cuda, oracle, case):
+    """Spot lights with 8 x 8 maps of independent texels: footprints that reach past the map's edge read the edge
+    texels, with the 2 x 2 filter and with the 6 x 6 wide one (whose window clamps each texel to the edge)."""
+    from tests.test_lighting_ref64_cpu import shadowed_case
+
+    scene, cam, prep, clus, (transforms, maps, res, wide) = shadowed_case(oracle, case)
+    got = _gpu_shadowed(cuda, oracle, scene, cam, prep, transforms, maps, res, pcf_wide=wide)
+    _compare(got, oracle.deferred_lighting_shadowed(scene, cam, prep, clus, transforms, maps, res, pcf_wide=wide), 0.97)
+    share = R.assert_meets_bar(got, R.reference(oracle, scene, cam, prep, clus, shadows=(transforms, maps, res, wide)), case)
+    print(f"{case}: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
 
 
 def test_cuda_shadowed_lighting_vs_reference_shader_fixture(cuda, oracle):
@@ -116,5 +138,8 @@ def test_viewer_frame_with_shadowed_lights(cuda, oracle):
     transforms = oracle.shadow_transforms(prep)
     assert np.array_equal(v.shadow_transforms(), transforms)
     ref = oracle.deferred_lighting_shadowed(scene, cam, prep, clus, transforms, maps, res)
-    _compare(v.download_image("HDR-main"), ref, 0.97)
+    got = v.download_image("HDR-main")
+    _compare(got, ref, 0.97)
+    share = R.assert_meets_bar(got, R.reference(oracle, scene, cam, prep, clus, shadows=(transforms, maps, res)), "viewer frame")
+    print(f"viewer frame: within the float64 bar; it admits one code on {share:.4f} of the lit channels")
     v.close()
