@@ -323,9 +323,18 @@ Image::Image(Device &device_, const ImageCreateInfo &info_) : device(device_), i
 	data = device.allocate(size);
 }
 
+Image::Image(Device &device_, const ImageCreateInfo &info_, void *external, unsigned row_pitch_)
+    : device(device_), info(info_), data(external), row_pitch(row_pitch_), owned(false)
+{
+	if (!format_texel_size(info.format) || !info.width || !info.height || !external || row_pitch < info.width * format_texel_size(info.format))
+		throw std::logic_error("granite_b200: bad external image");
+	size = (size_t)row_pitch * (info.height - 1) + (size_t)info.width * format_texel_size(info.format);
+}
+
 Image::~Image()
 {
-	device.free(data);
+	if (owned)
+		device.free(data);
 }
 
 Buffer::Buffer(Device &device_, const BufferCreateInfo &info_) : device(device_), info(info_)

@@ -41,6 +41,8 @@ class Image
 {
 public:
 	Image(Device &device, const ImageCreateInfo &info);
+	// Wraps memory the caller owns (a swapchain image): rows of row_pitch bytes; never freed here.
+	Image(Device &device, const ImageCreateInfo &info, void *external, unsigned row_pitch);
 	~Image();
 	Image(const Image &) = delete;
 	void operator=(const Image &) = delete;
@@ -51,6 +53,7 @@ public:
 	void *get_device_pointer() const { return data; }
 	size_t get_size() const { return size; }
 	unsigned get_row_pitch() const { return row_pitch; }
+	bool owns_memory() const { return owned; }
 
 private:
 	Device &device;
@@ -58,6 +61,7 @@ private:
 	void *data = nullptr;
 	size_t size = 0;
 	unsigned row_pitch = 0;
+	bool owned = true;
 };
 
 class ImageView

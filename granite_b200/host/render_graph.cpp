@@ -536,11 +536,15 @@ void RenderGraph::setup_attachments(Vulkan::Device &dev, Vulkan::ImageView *swap
 			continue;
 		if (i == backbuffer_physical && swapchain)
 		{
-			if (swapchain->get_view_width() != dim.width || swapchain->get_view_height() != dim.height)
+			if (swapchain->get_view_width() != dim.width || swapchain->get_view_height() != dim.height || swapchain->get_format() != dim.format)
 				throw std::logic_error("Swapchain image does not match the backbuffer dimensions.");
+			if (physical_attachments[i] && physical_attachments[i]->get_image().owns_memory())
+				forget_image(physical_attachments[i]->get_image()); // a graph-owned image, freed here
 			physical_attachments[i].reset(new Vulkan::ImageView(swapchain->get_image_handle()));
 			continue;
 		}
+		if (i == backbuffer_physical && physical_attachments[i] && !physical_attachments[i]->get_image().owns_memory())
+			physical_attachments[i].reset(); // the last frame went into a swapchain image: back to a graph-owned one
 		// history <-> current swap, renderer/render_graph.cpp:2706-2710
 		if (physical_has_history[i])
 			std::swap(physical_history_attachments[i], physical_attachments[i]);
@@ -608,6 +612,20 @@ void RenderGraph::enqueue_render_passes(Vulkan::Device &dev, TaskComposer &compo
 		pass_done_events.assign(passes.size(), std::array<Vulkan::Event, EventRing>{});
 	const unsigned slot = unsigned(frame_counter++ % EventRing);
 	unsigned errors = 0;
+	// the swapchain's events go to the first and the last pass that write the backbuffer
+	auto writes_backbuffer = [&](const RenderPass &pass) {
+		for (auto *w : pass.get_all_writes())
+			if (w->get_physical_index() == backbuffer_physical)
+				return true;
+		return false;
+	};
+	Vulkan::Event acquire = backbuffer_acquire, release = backbuffer_release;
+	backbuffer_acquire = backbuffer_release = nullptr;
+	unsigned last_backbuffer_writer = RenderResource::Unused;
+	if (release)
+		for (unsigned p : pass_stack)
+			if (writes_backbuffer(*passes[p]))
+				last_backbuffer_writer = p;
 	for (unsigned p : pass_stack)
 	{
 		auto &pass = *passes[p];
@@ -616,6 +634,11 @@ void RenderGraph::enqueue_render_passes(Vulkan::Device &dev, TaskComposer &compo
 			continue;
 		Vulkan::Stream stream = dev.get_queue_stream(queue_stream_index(pass.get_queue()));
 		Vulkan::CommandBuffer cmd(dev, stream);
+		if (acquire && writes_backbuffer(pass))
+		{
+			dev.stream_wait_event(stream, acquire);
+			acquire = nullptr;
+		}
 
 		const unsigned stream_index = queue_stream_index(pass.get_queue());
 		auto wait_for = [&](const void *key, bool writes) {
@@ -689,6 +712,8 @@ void RenderGraph::enqueue_render_passes(Vulkan::Device &dev, TaskComposer &compo
 			mark(physical_key(*w, false), true);
 		for (auto *h : pass.get_history_inputs())
 			mark(physical_key(*h, true), false);
+		if (p == last_backbuffer_writer)
+			dev.record_event_on(release, stream);
 		errors += cmd.get_error_count();
 	}
 	if (errors)

@@ -439,10 +439,21 @@ public:
 	void log();
 	// Allocates / reuses physical images and buffers, swaps history <-> current
 	// (render_graph.cpp:2686-2765).  `swapchain` may be null: the backbuffer source is then a
-	// graph-owned image of the backbuffer dimensions.
+	// graph-owned image of the backbuffer dimensions (allocated anew when the last frame's was `swapchain`).
 	void setup_attachments(Vulkan::Device &device, Vulkan::ImageView *swapchain);
 	// Records every baked pass, in order, on the device's stream.
 	void enqueue_render_passes(Vulkan::Device &device, TaskComposer &composer);
+	// The swapchain's acquire / render-complete pair for the next enqueue_render_passes only (either may be null): the
+	// stream of the first pass that writes the backbuffer waits on `acquire` before it, and `release` is recorded on
+	// the stream of the last one after it.
+	void set_backbuffer_events(Vulkan::Event acquire, Vulkan::Event release)
+	{
+		backbuffer_acquire = acquire;
+		backbuffer_release = release;
+	}
+	// Drops the cross-stream tracking of an image that no physical resource will hold again (a swapchain image that
+	// left the ring), so that its entry neither lingers nor passes to a later image at the same address.
+	void forget_image(const Vulkan::Image &image) { last_access.erase(&image); }
 
 	RenderTextureResource &get_texture_resource(const std::string &name);
 	RenderBufferResource &get_buffer_resource(const std::string &name);
@@ -546,6 +557,7 @@ private:
 	std::vector<std::unique_ptr<Vulkan::ImageView>> physical_history_spare;       // image to become "current" next frame
 	std::vector<Vulkan::BufferHandle> physical_buffers;
 	unsigned backbuffer_physical = RenderResource::Unused;
+	Vulkan::Event backbuffer_acquire = nullptr, backbuffer_release = nullptr;
 	bool baked = false;
 	// cross-stream ordering per physical resource: the last writer, and the last access (read or
 	// write) recorded on each of the three queue streams.  A reader waits for the writer; a writer

@@ -76,6 +76,13 @@ struct GrbhViewer
 	// row-sharded frames fed from the one rank that rasterises the whole frame (-1: off;
 	// grbh_viewer_set_gbuffer_source_rank): its "gbuffer" pass pushes every rank's input rows into that rank's slot
 	int gbuffer_source = -1;
+	// the caller's ring of output images (grbh_viewer_set_output_images), wrapped once each for the ring's life (the
+	// graph's cross-stream tracking keys on the wrapper), and the image, events of the next frame's acquire (-1: none)
+	std::vector<std::unique_ptr<Vulkan::ImageView>> output_ring;
+	int output_index = -1;
+	cudaEvent_t output_acquired = nullptr, output_rendered = nullptr;
+	// this frame's acquired image on the presenting rank: the "present" pass copies the assembled frame into it
+	Vulkan::ImageView *present_target = nullptr;
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
@@ -154,6 +161,23 @@ struct GrbhViewer
 		return { compute_shard_plan((unsigned)config.width, (unsigned)config.height, bands, q, uses_fxaa(), smaa_quality(), uses_taa(), shard_upscale()).lighting };
 	}
 	bool sharded_presenting() const { return bands.size() > 1 && present_rank >= 0; }
+	// the final pass's attachment format, which a ring image stands in for: EASU without RCAS stores UNORM codes
+	VkFormat output_format() const
+	{
+		if (config.hdr10_output)
+			return VK_FORMAT_A2B10G10R10_UNORM_PACK32;
+		return upscales() && !config.resolution_scale_sharpen ? VK_FORMAT_R8G8B8A8_UNORM : VK_FORMAT_R8G8B8A8_SRGB;
+	}
+	// a ring on a presenting layout belongs to the presenting rank only
+	std::string check_ring_rank(size_t count) const
+	{
+		if (count > 0 && sharded_presenting() && rank != (unsigned)present_rank)
+			return "rank " + std::to_string(rank) + " does not present (grbh_viewer_set_present_rank " + std::to_string(present_rank) +
+			       "): only the presenting rank may hold output images";
+		return "";
+	}
+	std::string check_output_images(const GrbImage *images, int32_t count) const;
+	void set_output_ring(const GrbImage *images, int32_t count);
 	bool fed_from_source() const { return bands.size() > 1 && gbuffer_source >= 0; }
 
 	// the G-buffer planes of the attachments (grb_gbuffer_copy_rows order), the G-buffer ones and / or motion vectors
@@ -206,6 +230,24 @@ struct GrbhViewer
 			record_consumed(stream, *pending_device);
 	}
 	void feed_from_source(Vulkan::CommandBuffer &cmd);
+
+	// the presenting rank with an acquired output image: the assembled frame (`presented`, laid out as `frame`) into
+	// it, behind the present pass on its stream, between the caller's two events
+	void copy_presented(Vulkan::CommandBuffer &cmd, const GrbImage &frame)
+	{
+		if (!present_target)
+			return;
+		auto stream = reinterpret_cast<cudaStream_t>(cmd.get_stream());
+		if (output_acquired)
+			Vulkan::cuda_ok(cudaStreamWaitEvent(stream, output_acquired, 0), "cudaStreamWaitEvent(acquired)");
+		const GrbImage dst = present_target->as_grb();
+		if (!Vulkan::cuda_ok(cudaMemcpy2DAsync(dst.data, (size_t)dst.row_pitch, presented, (size_t)frame.row_pitch, (size_t)frame.width * 4,
+		                                       (size_t)frame.height, cudaMemcpyDeviceToDevice, stream),
+		                     "present: copy into the output image"))
+			throw std::runtime_error("present: the copy into the acquired output image failed");
+		if (output_rendered)
+			Vulkan::cuda_ok(cudaEventRecord(output_rendered, stream), "cudaEventRecord(rendered)");
+	}
 
 	// the device-to-host copy of this rank's rows of the final image (the whole frame on the presenting rank), on the
 	// stream of the pass that produced it
@@ -566,12 +608,14 @@ void GrbhViewer::bake_render_graph()
 				{
 					cmd.check(grb_peer_wait(slot.flags[rank], (int32_t)slot.count, slot.epoch, stream), "grb_peer_wait");
 					presented = slot.images[P];
+					copy_presented(cmd, image);
 				}
 				return;
 			}
 			// without peer memory: every rank's band to every rank, in place (the output image is full-size everywhere)
 			graph.get_collectives()->all_gather_rows(cmd, view_, bands);
 			presented = image.data;
+			copy_presented(cmd, image);
 		});
 		ui_source = "presented";
 	}
@@ -620,6 +664,61 @@ std::string GrbhViewer::check_device_gbuffer(const GrbhDeviceGBuffer &g) const
 			       " bytes) and at least width x texel (" + std::to_string(w * p.texel) + ")";
 	}
 	return "";
+}
+
+std::string GrbhViewer::check_output_images(const GrbImage *images, int32_t count) const
+{
+	if (count < 0 || (count > 0 && !images))
+		return "bad arguments (count " + std::to_string(count) + (images ? ")" : ", images NULL)");
+	const int w = config.width, h = config.height;
+	const int32_t format = config.hdr10_output ? GRB_FORMAT_A2B10G10R10_UNORM_PACK32 : GRB_FORMAT_R8G8B8A8_SRGB;
+	for (int32_t i = 0; i < count; i++)
+	{
+		const GrbImage &im = images[i];
+		const std::string name = "output image " + std::to_string(i);
+		if (!im.data)
+			return name + " has no memory";
+		if (im.width != w || im.height != h)
+			return name + " is " + std::to_string(im.width) + " x " + std::to_string(im.height) + "; the display size is " + std::to_string(w) + " x " +
+			       std::to_string(h);
+		if (im.format != format)
+			return name + " has format " + std::to_string(im.format) + "; the viewer's output format is " + std::to_string(format) +
+			       (config.hdr10_output ? " (A2B10G10R10_UNORM_PACK32: HDR10 output)" : " (R8G8B8A8_SRGB)");
+		if (im.row_pitch < w * 4 || im.row_pitch % 16 != 0)
+			return name + "'s row_pitch " + std::to_string(im.row_pitch) + " must be a multiple of 16 bytes and at least width x 4 (" + std::to_string(w * 4) + ")";
+		if (reinterpret_cast<uintptr_t>(im.data) % 16 != 0)
+			return name + "'s base address is not 16-byte aligned";
+	}
+	// each image's bytes from its first texel to its last, as the final kernels may write them
+	auto span = [&](const GrbImage &im) {
+		const uintptr_t b = reinterpret_cast<uintptr_t>(im.data);
+		return std::make_pair(b, b + (uintptr_t)im.row_pitch * (uintptr_t)(h - 1) + (uintptr_t)w * 4);
+	};
+	for (int32_t i = 0; i < count; i++)
+		for (int32_t j = i + 1; j < count; j++)
+		{
+			const auto a = span(images[i]), b = span(images[j]);
+			if (a.first < b.second && b.first < a.second)
+				return "output images " + std::to_string(i) + " and " + std::to_string(j) + " overlap";
+		}
+	return check_ring_rank((size_t)count);
+}
+
+void GrbhViewer::set_output_ring(const GrbImage *images, int32_t count)
+{
+	// the caller may free an image of the old ring once its last frame's `rendered` event has completed: nothing of
+	// it stays in the graph's tracking
+	for (const auto &view_ : output_ring)
+		graph.forget_image(view_->get_image());
+	output_ring.clear();
+	output_index = -1;
+	output_acquired = output_rendered = nullptr;
+	Vulkan::ImageCreateInfo info;
+	info.width = (unsigned)config.width;
+	info.height = (unsigned)config.height;
+	info.format = output_format();
+	for (int32_t i = 0; i < count; i++)
+		output_ring.emplace_back(new Vulkan::ImageView(std::make_shared<Vulkan::Image>(*device, info, images[i].data, (unsigned)images[i].row_pitch)));
 }
 
 // Feeding from the rank S that rasterised the whole frame (DESIGN.md section 5, "Feeding a sharded frame from one
@@ -716,19 +815,22 @@ cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
 	if (bands_moved)
 		throw std::runtime_error("output readback: the bands moved (grbh_viewer_move_row_shards) since the last frame; render a frame first");
 	auto &output = graph.get_texture_resource(output_name);
-	const void *base = graph.get_physical_texture_resource(output).get_image().get_device_pointer();
+	// the graph-owned output image, or the caller's image the last frame went into (any pitch)
+	const Vulkan::Image &image = graph.get_physical_texture_resource(output).get_image();
+	const void *base = image.get_device_pointer();
+	size_t src_pitch = image.get_row_pitch();
 	r = bands.size() > 1 ? bands[rank] : GrbRows{ 0, config.height };
 	if (sharded_presenting() && rank == (unsigned)present_rank)
 	{
 		if (!presented)
 			throw std::runtime_error("output readback: no frame has been presented since the last bake");
-		base = presented; // the same size and pitch as the output image
+		base = presented; // the same size and pitch as the graph-owned output image
 		r = GrbRows{ 0, config.height };
 	}
 	const size_t pitch = (size_t)config.width * 4;
 	auto stream = reinterpret_cast<cudaStream_t>(graph.get_writer_stream(output));
-	if (!Vulkan::cuda_ok(cudaMemcpyAsync(reinterpret_cast<uint8_t *>(dst) + (size_t)r.y0 * pitch, static_cast<const uint8_t *>(base) + (size_t)r.y0 * pitch,
-	                                     pitch * (size_t)(r.y1 - r.y0), cudaMemcpyDeviceToHost, stream),
+	if (!Vulkan::cuda_ok(cudaMemcpy2DAsync(reinterpret_cast<uint8_t *>(dst) + (size_t)r.y0 * pitch, pitch, static_cast<const uint8_t *>(base) + (size_t)r.y0 * src_pitch,
+	                                       src_pitch, pitch, (size_t)(r.y1 - r.y0), cudaMemcpyDeviceToHost, stream),
 	                     "output readback"))
 		throw std::runtime_error("cudaMemcpyAsync failed");
 	return stream;
@@ -784,9 +886,13 @@ void GrbhViewer::render_frame(const GrbhHostGBuffer *host, double frame_time)
 	frame.elapsed_time += frame_time;
 	context.set_frame_parameters(frame);
 
+	// an acquired ring image: the backbuffer itself, or on the presenting rank the target of the present pass's copy
+	Vulkan::ImageView *acquired = output_index >= 0 ? output_ring[(size_t)output_index].get() : nullptr;
+	output_index = -1;
+	const bool bind = acquired && !sharded_presenting();
 	{
 		Vulkan::ScopedHostTimer timer("frame.setup_attachments");
-		graph.setup_attachments(*device, nullptr);
+		graph.setup_attachments(*device, bind ? acquired : nullptr);
 		cluster.setup_render_pass_resources(graph);
 	}
 
@@ -801,11 +907,24 @@ void GrbhViewer::render_frame(const GrbhHostGBuffer *host, double frame_time)
 	}
 
 	pending_upload = host;
+	present_target = bind ? nullptr : acquired;
+	if (bind)
+		graph.set_backbuffer_events(output_acquired, output_rendered);
 	{
 		Vulkan::ScopedHostTimer timer("frame.enqueue_render_passes");
-		graph.enqueue_render_passes(*device, composer);
+		try
+		{
+			graph.enqueue_render_passes(*device, composer);
+		}
+		catch (...)
+		{
+			pending_upload = nullptr;
+			present_target = nullptr;
+			throw;
+		}
 	}
 	pending_upload = nullptr;
+	present_target = nullptr;
 	profiled_frames++;
 
 	if (config.timestamps == 1)
@@ -1303,6 +1422,9 @@ extern "C" int32_t grbh_viewer_bake(GrbhViewer *v)
 {
 	if (!v)
 		return fail("null viewer");
+	const std::string ring_rank = v->check_ring_rank(v->output_ring.size());
+	if (!ring_rank.empty())
+		return fail("grbh_viewer_bake: " + ring_rank + " (grbh_viewer_set_output_images with count 0 drops them)");
 	if (!v->device)
 		return fail("grbh_viewer_bake: host-only viewer (cuda_device < 0) cannot bake");
 	GRBH_TRY
@@ -1314,8 +1436,67 @@ extern "C" int32_t grbh_viewer_bake(GrbhViewer *v)
 	GRBH_CATCH
 }
 
+extern "C" int32_t grbh_viewer_set_output_images(GrbhViewer *v, const GrbImage *images, int32_t count)
+{
+	const char *fn = "grbh_viewer_set_output_images: ";
+	if (!v)
+		return fail(std::string(fn) + "null viewer");
+	const std::string bad = v->check_output_images(images, count);
+	if (!bad.empty())
+		return fail(fn + bad);
+	if (count > 0 && !v->device)
+		return fail(std::string(fn) + "host-only viewer (cuda_device < 0) has no device for the images to be on");
+	GRBH_TRY
+	for (int32_t i = 0; i < count; i++)
+	{
+		// the first and the last byte of each image are device memory of the viewer's device
+		const uint8_t *base = static_cast<const uint8_t *>(images[i].data);
+		for (const uint8_t *p : { base, base + (size_t)images[i].row_pitch * (size_t)(images[i].height - 1) + (size_t)images[i].width * 4 - 1 })
+		{
+			cudaPointerAttributes attr = {};
+			const cudaError_t err = cudaPointerGetAttributes(&attr, p);
+			if (err != cudaSuccess)
+				cudaGetLastError();
+			if (err != cudaSuccess || (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) ||
+			    attr.device != v->device->get_device_index())
+				return fail(std::string(fn) + "output image " + std::to_string(i) + " is not device memory of the viewer's device (" +
+				            std::to_string(v->device->get_device_index()) + ")");
+		}
+	}
+	v->set_output_ring(images, count);
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_acquire_output(GrbhViewer *v, int32_t index, void *acquired, void *rendered)
+{
+	const char *fn = "grbh_viewer_acquire_output: ";
+	if (!v)
+		return fail(std::string(fn) + "null viewer");
+	if (v->output_ring.empty())
+		return fail(std::string(fn) + "no output images are set (grbh_viewer_set_output_images)");
+	if (index < 0 || (size_t)index >= v->output_ring.size())
+		return fail(std::string(fn) + "index " + std::to_string(index) + " is out of range: the ring holds " + std::to_string(v->output_ring.size()) +
+		            " images");
+	v->output_index = index;
+	v->output_acquired = static_cast<cudaEvent_t>(acquired);
+	v->output_rendered = static_cast<cudaEvent_t>(rendered);
+	return 0;
+}
+
+// While a ring of output images is set, every frame renders into an acquired one
+static bool frame_without_acquire(const GrbhViewer *v, const char *fn)
+{
+	if (v->output_ring.empty() || v->output_index >= 0)
+		return false;
+	fail(std::string(fn) + "a ring of output images is set (grbh_viewer_set_output_images): grbh_viewer_acquire_output must precede every frame");
+	return true;
+}
+
 extern "C" int32_t grbh_viewer_render_frame(GrbhViewer *v, const GrbhHostGBuffer *host, double frame_time)
 {
+	if (v && frame_without_acquire(v, "grbh_viewer_render_frame: "))
+		return -1;
 	if (v && v->fed_from_source())
 		return fail("grbh_viewer_render_frame: the frame is fed from the G-buffer source rank (grbh_viewer_set_gbuffer_source_rank); every rank calls "
 		            "grbh_viewer_render_frame_device");
@@ -1340,6 +1521,8 @@ extern "C" int32_t grbh_viewer_render_frame_device(GrbhViewer *v, const GrbhDevi
 	const char *fn = "grbh_viewer_render_frame_device: ";
 	if (!v)
 		return fail(std::string(fn) + "null viewer");
+	if (frame_without_acquire(v, fn))
+		return -1;
 	if (v->fed_from_source())
 	{
 		const bool source = v->rank == (unsigned)v->gbuffer_source;

@@ -61,6 +61,8 @@ def lib() -> C.CDLL:
         _lib.grbh_viewer_render_frame_device.argtypes = [C.c_void_p, C.POINTER(GrbhDeviceGBuffer), C.c_double]
         _lib.grbh_viewer_get_input_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         _lib.grbh_viewer_set_exposure.argtypes = [C.c_void_p, C.c_float]
+        _lib.grbh_viewer_set_output_images.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
+        _lib.grbh_viewer_acquire_output.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -321,6 +323,7 @@ class Viewer:
         cfg.volumetric_decals = int(volumetric_decals)
         cfg.render_target_fp16 = int(render_target_fp16)  # emissive / HDR-main as RGBA16F: host_gbuffer's emissive is (H, W, 4) uint16
         self.width, self.height = width, height
+        self._hdr10 = bool(hdr10_output)
         self._h = C.c_void_p()
         _check(lib().grbh_viewer_create(C.byref(cfg), C.byref(self._h)), "grbh_viewer_create")
         self._keep = []
@@ -476,6 +479,26 @@ class Viewer:
             arg.consumed = None if consumed is None else consumed.cuda_event
             arg = C.byref(arg)
         _check(lib().grbh_viewer_render_frame_device(self._h, arg, C.c_double(frame_time)), "grbh_viewer_render_frame_device")
+
+    def set_output_images(self, tensors):
+        """A ring of caller-owned output images that frames render into instead of the graph-owned one
+        (grbh_viewer_set_output_images): torch tensors on the viewer's device, each an (H, W) int32 view at the display
+        size of any row stride (a multiple of 16 bytes, 16-byte aligned).  [] goes back to the graph-owned image.  The
+        tensors must stay alive until the `rendered` event of their last frame has completed."""
+        fmt = capi.FORMAT_A2B10G10R10_UNORM if self._hdr10 else capi.FORMAT_R8G8B8A8_SRGB
+        images = [capi.pitched_image(t, fmt) for t in tensors]
+        arr = (capi.GrbImage * max(len(images), 1))(*images)
+        _check(lib().grbh_viewer_set_output_images(self._h, arr, len(images)), "grbh_viewer_set_output_images")
+        self._ring = list(tensors)
+
+    def acquire_output(self, index, acquired=None, rendered=None):
+        """The next frame renders into ring image `index` (grbh_viewer_acquire_output).  acquired: a torch.cuda.Event
+        the frame waits on before its first write to the image; rendered: a torch.cuda.Event the viewer records after
+        its last write."""
+        if rendered is not None and not rendered.cuda_event:
+            rendered.record()  # torch creates the CUDA event on its first record
+        _check(lib().grbh_viewer_acquire_output(self._h, int(index), None if acquired is None else (acquired.cuda_event or None),
+                                                None if rendered is None else rendered.cuda_event), "grbh_viewer_acquire_output")
 
     def read_output(self, dst):
         """dst: full-frame uint32 buffer (numpy array or pinned torch tensor). Returns the (y0, y1) band written."""

@@ -258,9 +258,30 @@ int32_t grbh_viewer_render_frame(GrbhViewer *viewer, const GrbhHostGBuffer *host
  * attachment's format, a pitch too small or not a multiple of the texel size, a host-only viewer; and under
  * grbh_viewer_set_gbuffer_source_rank a NULL G-buffer on the source rank or a G-buffer on any other. */
 int32_t grbh_viewer_render_frame_device(GrbhViewer *viewer, const GrbhDeviceGBuffer *gbuffer, double frame_time);
+/* A ring of `count` caller-owned device images that frames render into, in place of the graph-owned output image (the
+ * reference's swapchain / headless image ring).  Each image: the display size (width x height, also under FSR 1), the
+ * viewer's output format (R8G8B8A8_SRGB; A2B10G10R10_UNORM_PACK32 with hdr10_output), base 16-byte aligned, row_pitch a
+ * multiple of 16 and >= width * 4, device memory of the viewer's device, no two overlapping.  The bytes written are the
+ * ones grbh_viewer_read_output returns without a ring, bit for bit (FSR 1 without RCAS stores UNORM codes, as there).
+ * count = 0: back to the graph-owned image.  May be called between frames; takes effect at the next
+ * grbh_viewer_acquire_output (an acquire of the old ring is dropped).  An image of the old ring may be freed once the
+ * `rendered` event of its last frame has completed.
+ * One GPU, or a row-sharded rank without a presenting rank: the acquired image is the backbuffer, and the final pass
+ * writes into it directly (on a row-sharded rank only the band's rows; the others stay as they are).
+ * A presenting row-sharded viewer (grbh_viewer_set_present_rank): only the presenting rank may hold images (refused here
+ * and at bake on every other rank); its backbuffer stays graph-owned, and after the "present" pass, on its stream, the
+ * assembled frame is copied into the acquired image (DESIGN.md section 5, "Presenting a sharded frame"). */
+int32_t grbh_viewer_set_output_images(GrbhViewer *viewer, const GrbImage *images, int32_t count);
+/* The next frame renders into images[index] of the ring.  acquired: an event (cudaEvent_t, or NULL) the frame waits on
+ * before its first write to that image (the caller's last reads of it are done).  rendered: a caller-created event (or
+ * NULL) the viewer records after the frame's last write to it.  Both on the stream of the pass that writes the image.
+ * While a ring is set, every grbh_viewer_render_frame / _device must follow an acquire; a frame without one is refused
+ * before anything is recorded. */
+int32_t grbh_viewer_acquire_output(GrbhViewer *viewer, int32_t index, void *acquired, void *rendered);
 /* Copies this rank's rows of the final image (R8G8B8A8) to host memory laid out as the full
  * frame (row pitch = width*4) and waits for it. rows_out receives the band (the whole frame on
- * the presenting rank, grbh_viewer_set_present_rank). */
+ * the presenting rank, grbh_viewer_set_present_rank).  With a ring of output images: the image
+ * the last frame went into. */
 int32_t grbh_viewer_read_output(GrbhViewer *viewer, uint32_t *dst_full_frame, GrbRows *rows_out);
 /* Asynchronous form: enqueues the device->host copy of this frame's rows behind the frame and
  * returns; grbh_viewer_wait_outputs(viewer, k) blocks until at most k such copies are pending
