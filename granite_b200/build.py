@@ -19,6 +19,7 @@ COMMON += os.environ.get("GRB_EXTRA_NVCC_FLAGS", "").split()
 UNITS = [
     ("grb_api.cu", []),
     ("grb_cluster.cu", ["-fmad=false"]),
+    ("grb_light_prep.cu", ["-fmad=false"]),
     ("grb_post.cu", ["-fmad=false"]),
     ("grb_post_tiles.cu", ["-fmad=false"]),
     ("grb_post_fast.cu", []),

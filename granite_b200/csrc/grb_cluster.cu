@@ -343,8 +343,12 @@ __device__ __forceinline__ bool test_spot_light(float2 uv, float2 stride, const 
 // same tile block so a tile's words leave the CTA as one 16-byte segment.
 constexpr int kBinWarps = 4;
 
+// Counted: the list was prepared on the device and holds `*count` lights in its num_lights slots; the chunks at or
+// past ceil(count / 32) are stored as zero and the bits >= count are never set.
+template <bool Counted>
 __global__ void __launch_bounds__(32 * kBinWarps) binning_kernel(BinParams p, const uint32_t *__restrict__ type_mask,
-                                                                const float4 *__restrict__ cull_setup, uint32_t *__restrict__ bitmask)
+                                                                const float4 *__restrict__ cull_setup, uint32_t *__restrict__ bitmask,
+                                                                const int32_t *__restrict__ count)
 {
 	const int lane = threadIdx.x & 31;
 	const int warp = threadIdx.x >> 5;
@@ -352,6 +356,15 @@ __global__ void __launch_bounds__(32 * kBinWarps) binning_kernel(BinParams p, co
 	const int bx = blockIdx.y, by = p.first_block_y + blockIdx.z;
 	if (chunk >= p.num_lights_32)
 		return;
+	if (Counted)
+	{
+		p.num_lights = min(__ldg(count), p.num_lights);
+		if (chunk * 32 >= p.num_lights)
+		{
+			bitmask[((size_t)(by * 4 + (lane >> 3)) * p.res_x + bx * 8 + (lane & 7)) * p.num_lights_32 + chunk] = 0u;
+			return;
+		}
+	}
 
 	float2 tile_uv = make_float2(2.0f * (float)(bx * 8) * p.inv_res.x - 1.0f, 2.0f * (float)(by * 4) * p.inv_res.y - 1.0f);
 	float2 tile_stride = make_float2((2.0f * 8.0f) * p.inv_res.x, (2.0f * 4.0f) * p.inv_res.y);
@@ -546,7 +559,9 @@ extern "C" int32_t grb_cluster_cull_setup(const GrbCamera *cam, const GrbCluster
 	return check_launch("grb_cluster_cull_setup");
 }
 
-extern "C" int32_t grb_cluster_binning_rows(const GrbClusterParameters *params, const GrbClusterBuffers *buf, int32_t tile_y0, int32_t tile_y1, void *stream)
+namespace
+{
+int32_t binning_rows(const GrbClusterParameters *params, const GrbClusterBuffers *buf, const int32_t *count, int32_t tile_y0, int32_t tile_y1, void *stream)
 {
 	if (!args_ok(params, buf, "grb_cluster_binning: bad parameters (resolution must be a multiple of 8x4)"))
 		return GRB_ERR_INVALID_ARGUMENT;
@@ -575,8 +590,29 @@ extern "C" int32_t grb_cluster_binning_rows(const GrbClusterParameters *params, 
 		return GRB_OK;
 	p.first_block_y = by0;
 	dim3 grid((p.num_lights_32 + kBinWarps - 1) / kBinWarps, p.res_x / 8, by1 - by0);
-	binning_kernel<<<grid, 32 * kBinWarps, 0, as_stream(stream)>>>(p, buf->type_mask, reinterpret_cast<const float4 *>(buf->cull_setup), buf->bitmask);
+	const float4 *cull = reinterpret_cast<const float4 *>(buf->cull_setup);
+	if (count)
+		binning_kernel<true><<<grid, 32 * kBinWarps, 0, as_stream(stream)>>>(p, buf->type_mask, cull, buf->bitmask, count);
+	else
+		binning_kernel<false><<<grid, 32 * kBinWarps, 0, as_stream(stream)>>>(p, buf->type_mask, cull, buf->bitmask, nullptr);
 	return check_launch("grb_cluster_binning");
+}
+} // namespace
+
+extern "C" int32_t grb_cluster_binning_rows(const GrbClusterParameters *params, const GrbClusterBuffers *buf, int32_t tile_y0, int32_t tile_y1, void *stream)
+{
+	return binning_rows(params, buf, nullptr, tile_y0, tile_y1, stream);
+}
+
+extern "C" int32_t grb_cluster_binning_rows_counted(const GrbClusterParameters *params, const GrbClusterBuffers *buf, const int32_t *device_count,
+                                                    int32_t tile_y0, int32_t tile_y1, void *stream)
+{
+	if (!device_count)
+	{
+		set_last_error("grb_cluster_binning_rows_counted: null device_count");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return binning_rows(params, buf, device_count, tile_y0, tile_y1, stream);
 }
 
 extern "C" int32_t grb_cluster_binning(const GrbClusterParameters *params, const GrbClusterBuffers *buf, void *stream)

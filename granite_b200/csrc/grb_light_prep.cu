@@ -1,0 +1,167 @@
+// grb_light_prep.cu -- LightClusterer::refresh_bindless_prepare for a light list that lives in device memory: frustum
+// cull, front-to-back sort and packing into the "cluster-transforms" layout, with the kept count left on the device.
+// Compiled with -fmad=false: the per-light arithmetic (grb_light_prep.cuh) must round every operation as the host
+// prep does, so the packed bytes are the host's.
+//
+// Three steps on the caller's stream:
+//   1. cull_key_kernel, one thread per input light: visibility and a 33-bit sort key (bit 32 = culled, bits 0..31 the
+//      order-preserving code of dot(position, camera_front)) with the light's index as the value;
+//   2. cub::DeviceRadixSort::SortPairs over those 33 bits -- stable, so equal keys keep input order, which is the host's
+//      by_key_then_input comparator;
+//   3. pack_kernel, one thread per slot of GRB_MAX_CLUSTER_LIGHTS: the visible count is where the culled keys begin
+//      (a binary search of the sorted keys), and slot s < count packs sorted light s.
+#include "grb_common.cuh"
+#include "grb_light_prep.cuh"
+
+#include <cub/device/device_radix_sort.cuh>
+
+namespace grb
+{
+namespace
+{
+constexpr int kMaxInputLights = 65536;
+constexpr int kPackThreads = 256;
+
+__global__ void __launch_bounds__(256) cull_key_kernel(GrbLightList lights, GrbLightPrepView view, unsigned long long *__restrict__ keys,
+                                                       uint32_t *__restrict__ values)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= lights.count)
+		return;
+	const lp::Light L = lp::load_light(lights, i);
+	const bool vis = !view.frustum_culling || lp::visible(L, view.planes);
+	keys[i] = ((unsigned long long)(vis ? 0u : 1u) << 32) | lp::radix_key(lp::sort_key(L, view.camera_front));
+	values[i] = (uint32_t)i;
+}
+
+__global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights, GrbLightPrepView view, const unsigned long long *__restrict__ keys,
+                                                           const uint32_t *__restrict__ order, GrbPositionalLight *__restrict__ records,
+                                                           float *__restrict__ model, uint32_t *__restrict__ type_mask, uint2 *__restrict__ z_ranges,
+                                                           int32_t *__restrict__ count_out)
+{
+	__shared__ int s_count;
+	if (threadIdx.x == 0)
+	{
+		// the sorted keys hold the visible lights first: the count is the first culled key's index
+		int lo = 0, hi = lights.count;
+		while (lo < hi)
+		{
+			const int mid = (lo + hi) >> 1;
+			if (keys[mid] >> 32)
+				hi = mid;
+			else
+				lo = mid + 1;
+		}
+		s_count = min(lo, GRB_MAX_CLUSTER_LIGHTS);
+	}
+	__syncthreads();
+	const int count = s_count;
+	const int slots = min(lights.count, GRB_MAX_CLUSTER_LIGHTS);
+	const int s = blockIdx.x * blockDim.x + threadIdx.x;
+	bool point = false;
+	if (s < count)
+	{
+		const lp::Light L = lp::load_light(lights, (int)order[s]);
+		GrbPositionalLight rec;
+		float m[12];
+		uint32_t zr[2];
+		lp::pack(L, view, rec, m, zr);
+		records[s] = rec;
+		for (int k = 0; k < 12; k++)
+			model[12 * s + k] = m[k];
+		z_ranges[s] = make_uint2(zr[0], zr[1]);
+		point = L.point;
+	}
+	else if (s < max(slots, 1))
+	{
+		if (s < slots)
+		{
+			records[s] = GrbPositionalLight{};
+			for (int k = 0; k < 12; k++)
+				model[12 * s + k] = 0.0f;
+		}
+		z_ranges[s] = make_uint2(0xffffffffu, 0u);
+	}
+	// one type-mask word per warp: every word of the mask is written, zero past the kept lights
+	const uint32_t word = __ballot_sync(0xffffffffu, point);
+	if ((threadIdx.x & 31) == 0)
+		type_mask[s >> 5] = word;
+	if (s == 0)
+		*count_out = count;
+}
+
+struct ScratchLayout
+{
+	size_t keys_in, keys_out, values_in, values_out, temp, temp_bytes, total;
+};
+
+size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
+
+bool scratch_layout(int n, ScratchLayout &l)
+{
+	l.temp_bytes = 0;
+	if (n > 0 && cub::DeviceRadixSort::SortPairs(nullptr, l.temp_bytes, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+	                                              (const uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, 33) != cudaSuccess)
+		return false;
+	const size_t n8 = align256((size_t)n * 8), n4 = align256((size_t)n * 4);
+	l.keys_in = 0;
+	l.keys_out = n8;
+	l.values_in = 2 * n8;
+	l.values_out = 2 * n8 + n4;
+	l.temp = 2 * n8 + 2 * n4;
+	l.total = l.temp + align256(l.temp_bytes);
+	return true;
+}
+} // namespace
+} // namespace grb
+
+using namespace grb;
+
+extern "C" uint64_t grb_light_prep_scratch_bytes(int32_t max_lights)
+{
+	ScratchLayout l;
+	if (max_lights < 0 || max_lights > kMaxInputLights || !scratch_layout(max_lights, l))
+	{
+		cudaGetLastError();
+		return 0;
+	}
+	return l.total;
+}
+
+extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
+                                  uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+{
+	if (!lights || !view || !records || !model || !type_mask || !z_ranges || !device_count || lights->count < 0 || lights->count > kMaxInputLights ||
+	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone ||
+	                           !lights->outer_cone || !scratch)))
+	{
+		set_last_error("grb_light_prep: a null pointer or a count outside 0..65536");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	const int n = lights->count;
+	ScratchLayout l;
+	if (!scratch_layout(n, l))
+		return check_launch("grb_light_prep: radix sort size");
+	if (scratch_bytes < l.total)
+	{
+		set_last_error("grb_light_prep: scratch smaller than grb_light_prep_scratch_bytes(count)");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	auto *base = static_cast<uint8_t *>(scratch);
+	auto *keys_in = reinterpret_cast<unsigned long long *>(base + l.keys_in), *keys_out = reinterpret_cast<unsigned long long *>(base + l.keys_out);
+	auto *values_in = reinterpret_cast<uint32_t *>(base + l.values_in), *values_out = reinterpret_cast<uint32_t *>(base + l.values_out);
+	cudaStream_t s = as_stream(stream);
+	if (n > 0)
+	{
+		cull_key_kernel<<<(n + 255) / 256, 256, 0, s>>>(*lights, *view, keys_in, values_in);
+		int32_t r = check_launch("grb_light_prep: cull");
+		if (r != GRB_OK)
+			return r;
+		size_t temp_bytes = l.temp_bytes;
+		if (cub::DeviceRadixSort::SortPairs(base + l.temp, temp_bytes, keys_in, keys_out, values_in, values_out, n, 0, 33, s) != cudaSuccess)
+			return check_launch("grb_light_prep: sort");
+	}
+	pack_kernel<<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, *view, keys_out, values_out, records, model, type_mask,
+	                                                                              reinterpret_cast<uint2 *>(z_ranges), device_count);
+	return check_launch("grb_light_prep: pack");
+}

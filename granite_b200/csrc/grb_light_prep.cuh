@@ -1,0 +1,279 @@
+// grb_light_prep.cuh -- the per-light arithmetic of the host light prep (LightClusterer::refresh_bindless_prepare with
+// PositionalLight / PointLight / SpotLight, AABB::transform, Frustum::intersects_fast, compute_uint_range) restated as
+// __host__ __device__ functions over one light of a GrbLightList.  Every fp32 operation is written in the host code's
+// association order; the device build uses -fmad=false and the host build -ffp-contract=off, so both round each
+// operation on its own and give the host prep's bytes.  No transcendentals: + - * /, sqrtf, compares, floatToHalf.
+#pragma once
+
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+#include "../../include/granite_b200.h"
+
+namespace grb
+{
+namespace lp
+{
+struct V3
+{
+	float x, y, z;
+};
+
+__host__ __device__ inline uint32_t bits(float f)
+{
+	uint32_t u;
+	memcpy(&u, &f, 4);
+	return u;
+}
+__host__ __device__ inline V3 add(V3 a, V3 b) { return V3{ a.x + b.x, a.y + b.y, a.z + b.z }; }
+__host__ __device__ inline V3 sub(V3 a, V3 b) { return V3{ a.x - b.x, a.y - b.y, a.z - b.z }; }
+__host__ __device__ inline float dot(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+// muglm's min / max: the first argument wins only on a strict compare
+__host__ __device__ inline float mn(float a, float b) { return a < b ? a : b; }
+__host__ __device__ inline float mx(float a, float b) { return a > b ? a : b; }
+
+// muglm::floatToHalf (host/math.cpp): round half up on the magnitude
+__host__ __device__ inline uint16_t float_to_half(float v)
+{
+	const uint32_t u = bits(v);
+	const uint32_t sign = (u >> 16) & 0x8000u;
+	const uint32_t mag = u & 0x7fffffffu;
+	if (mag >= 0x7f800000u)
+	{
+		uint32_t payload = (mag & 0x7fffffu) >> 13;
+		if ((mag & 0x7fffffu) != 0 && payload == 0)
+			payload = 1;
+		return (uint16_t)(sign | 0x7c00u | payload);
+	}
+	const int e = (int)(mag >> 23) - 112;
+	if (e <= 0)
+	{
+		if (e < -10)
+			return (uint16_t)sign;
+		uint32_t m = ((mag & 0x7fffffu) | 0x800000u) >> (1 - e);
+		return (uint16_t)(sign | ((m + 0x1000u) >> 13));
+	}
+	uint32_t h = (((uint32_t)e << 23) | (mag & 0x7fffffu)) + 0x1000u;
+	h >>= 13;
+	if (h >= 0x7c00u)
+		h = 0x7c00u;
+	return (uint16_t)(sign | h);
+}
+
+// One input light as the viewer's grbh_viewer_set_lights builds it: the node transform's three rows (a point light's
+// rotation is the identity) and the PositionalLight state after set_maximum_range, set_color and, for a spot light,
+// set_spot_parameters.
+struct Light
+{
+	float row[3][4];
+	V3 color;
+	bool point;
+	float inner, outer;  // clamped to [0.001, 1]
+	float falloff;       // recompute_range: sqrt(max channel / 0.1)
+	float reach;         // min(falloff, cutoff)
+	float xy_range;      // spot: tan of the outer half-angle
+	V3 lo, hi;           // the static AABB
+};
+
+__host__ __device__ inline Light load_light(const GrbLightList &l, int i)
+{
+	Light L;
+	const float *p = l.position + 3 * i;
+	L.color = V3{ l.color[3 * i], l.color[3 * i + 1], l.color[3 * i + 2] };
+	L.point = l.is_point[i] != 0;
+	if (L.point)
+	{
+		for (int c = 0; c < 3; c++)
+		{
+			for (int k = 0; k < 3; k++)
+				L.row[c][k] = c == k ? 1.0f : 0.0f;
+			L.row[c][3] = p[c];
+		}
+	}
+	else
+	{
+		const float *r = l.rotation + 9 * i; // column-major 3x3
+		for (int c = 0; c < 3; c++)
+		{
+			L.row[c][0] = r[c];
+			L.row[c][1] = r[3 + c];
+			L.row[c][2] = r[6 + c];
+			L.row[c][3] = p[c];
+		}
+	}
+	const float target_atten = 0.1f;
+	const float max_color = mx(mx(L.color.x, L.color.y), L.color.z);
+	L.falloff = sqrtf(max_color / target_atten);
+	L.reach = mn(L.falloff, l.cutoff_range);
+	L.inner = L.outer = 0.0f;
+	L.xy_range = 0.0f;
+	if (L.point)
+	{
+		L.lo = V3{ -L.reach, -L.reach, -L.reach };
+		L.hi = V3{ L.reach, L.reach, L.reach };
+	}
+	else
+	{
+		L.inner = mn(mx(l.inner_cone[i], 0.001f), 1.0f);
+		L.outer = mn(mx(l.outer_cone[i], 0.001f), 1.0f);
+		L.xy_range = sqrtf(1.0f - L.outer * L.outer) / L.outer;
+		const float side = L.xy_range * L.reach;
+		L.lo = V3{ -side, -side, -L.reach };
+		L.hi = V3{ side, side, 0.0f };
+	}
+	return L;
+}
+
+__host__ __device__ inline V3 translation(const Light &L) { return V3{ L.row[0][3], L.row[1][3], L.row[2][3] }; }
+
+// AABB::transform then Frustum::intersects_fast (std::signbit of the plane distance)
+__host__ __device__ inline bool visible(const Light &L, const float planes[24])
+{
+	float lo[3], hi[3];
+	const float mn_[3] = { L.lo.x, L.lo.y, L.lo.z }, mx_[3] = { L.hi.x, L.hi.y, L.hi.z };
+	for (int c = 0; c < 3; c++)
+	{
+		float h = L.row[c][3], l = L.row[c][3];
+		for (int k = 0; k < 3; k++)
+		{
+			const float m = L.row[c][k];
+			const bool positive = m > 0.0f;
+			h = h + m * (positive ? mx_[k] : mn_[k]);
+			l = l + m * (positive ? mn_[k] : mx_[k]);
+		}
+		hi[c] = h;
+		lo[c] = l;
+	}
+	for (int q = 0; q < 6; q++)
+	{
+		const float *p = planes + 4 * q;
+		const float dx = p[0] * (p[0] > 0.0f ? hi[0] : lo[0]);
+		const float dy = p[1] * (p[1] > 0.0f ? hi[1] : lo[1]);
+		const float dz = p[2] * (p[2] > 0.0f ? hi[2] : lo[2]);
+		const float dw = p[3] * 1.0f;
+		if (bits((dx + dy) + (dz + dw)) >> 31)
+			return false;
+	}
+	return true;
+}
+
+// dot(translation, camera_front): the front-to-back sort key
+__host__ __device__ inline float sort_key(const Light &L, const float front[3])
+{
+	return dot(translation(L), V3{ front[0], front[1], front[2] });
+}
+
+// The key as an unsigned integer that orders like the float's `<`: -0 and +0 compare equal, so both map to +0's code.
+__host__ __device__ inline uint32_t radix_key(float key)
+{
+	if (key == 0.0f)
+		key = 0.0f;
+	const uint32_t u = bits(key);
+	return (u >> 31) ? ~u : (u | 0x80000000u);
+}
+
+// PointLight / SpotLight::get_shader_info, the model row (set_point_model_transform / SpotLight::build_model_matrix) and
+// the Z-slice range (point_light_z_range / spot_light_z_range, then compute_uint_range)
+__host__ __device__ inline void pack(const Light &L, const GrbLightPrepView &view, GrbPositionalLight &rec, float model[12], uint32_t zr[2])
+{
+	const float scale_factor = sqrtf(L.row[0][0] * L.row[0][0] + L.row[0][1] * L.row[0][1] + L.row[0][2] * L.row[0][2]);
+	const float max_range = L.reach * scale_factor;
+	const float s2 = scale_factor * scale_factor;
+	rec.color[0] = L.color.x * s2;
+	rec.color[1] = L.color.y * s2;
+	rec.color[2] = L.color.z * s2;
+	for (int c = 0; c < 3; c++)
+		rec.position[c] = L.row[c][3];
+	V3 forward{ -L.row[0][2], -L.row[1][2], -L.row[2][2] };
+	if (L.point)
+	{
+		rec.spot_scale_bias[0] = rec.spot_scale_bias[1] = 0;
+		rec.offset_radius[0] = float_to_half(0.0f);
+		rec.offset_radius[1] = float_to_half(max_range);
+	}
+	else
+	{
+		const float spot_scale = 1.0f / mx(0.001f, L.inner - L.outer);
+		const float spot_bias = -L.outer * spot_scale;
+		const float tan2 = (1.0f - L.outer * L.outer) / (L.outer * L.outer);
+		const float center_distance = ((tan2 + 1.0f) * max_range) * 0.5f;
+		float spot_offset, spot_radius;
+		if (center_distance < max_range)
+		{
+			spot_offset = center_distance;
+			spot_radius = center_distance;
+		}
+		else
+		{
+			spot_offset = max_range;
+			spot_radius = sqrtf(tan2) * max_range;
+		}
+		rec.spot_scale_bias[0] = float_to_half(spot_scale);
+		rec.spot_scale_bias[1] = float_to_half(spot_bias);
+		rec.offset_radius[0] = float_to_half(spot_offset);
+		rec.offset_radius[1] = float_to_half(spot_radius);
+		const float inv_len = 1.0f / sqrtf(dot(forward, forward));
+		forward = V3{ forward.x * inv_len, forward.y * inv_len, forward.z * inv_len };
+	}
+	rec.direction[0] = forward.x;
+	rec.direction[1] = forward.y;
+	rec.direction[2] = forward.z;
+	rec.inv_radius = 1.0f / max_range;
+
+	const V3 cam{ view.camera_position[0], view.camera_position[1], view.camera_position[2] };
+	const V3 front{ view.camera_front[0], view.camera_front[1], view.camera_front[2] };
+	float lo, hi;
+	if (L.point)
+	{
+		const float radius = 1.0f / rec.inv_radius;
+		for (int k = 0; k < 12; k++)
+			model[k] = 0.0f;
+		model[0] = rec.position[0];
+		model[1] = rec.position[1];
+		model[2] = rec.position[2];
+		model[3] = radius;
+		const float z = dot(sub(translation(L), cam), front);
+		lo = z - radius;
+		hi = z + radius;
+	}
+	else
+	{
+		const float s[3] = { L.xy_range * L.reach, L.xy_range * L.reach, L.reach };
+		for (int c = 0; c < 3; c++)
+		{
+			for (int k = 0; k < 3; k++)
+				model[4 * c + k] = L.row[c][k] * s[k];
+			model[4 * c + 3] = L.row[c][3];
+		}
+		const V3 base{ model[3], model[7], model[11] };
+		const V3 x_off{ model[0], model[4], model[8] };
+		const V3 y_off{ model[1], model[5], model[9] };
+		const V3 z_base = add(base, V3{ -model[2], -model[6], -model[10] });
+		const V3 hull[5] = { base, add(add(z_base, x_off), y_off), add(sub(z_base, x_off), y_off), sub(add(z_base, x_off), y_off),
+			                 sub(sub(z_base, x_off), y_off) };
+		lo = INFINITY;
+		hi = -lo;
+		for (int k = 0; k < 5; k++)
+		{
+			const float z = dot(sub(hull[k], cam), front);
+			lo = mn(z, lo);
+			hi = mx(z, hi);
+		}
+	}
+	// compute_uint_range
+	float x = lo / view.z_slice_extent, y = hi / view.z_slice_extent;
+	if (y < 0.0f)
+	{
+		zr[0] = 0xffffffffu;
+		zr[1] = 0u;
+		return;
+	}
+	x = mx(x, 0.0f);
+	// float -> uint32 as the x86-64 host converts it: through a signed 64-bit truncation
+	zr[0] = (uint32_t)(int64_t)x;
+	const uint32_t uy = (uint32_t)(int64_t)y;
+	zr[1] = uy < (uint32_t)view.z_max_index ? uy : (uint32_t)view.z_max_index;
+}
+} // namespace lp
+} // namespace grb

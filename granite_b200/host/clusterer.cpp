@@ -302,7 +302,7 @@ void LightClusterer::refresh_bindless_prepare(const RenderContext &ctx)
 	// order, is deterministic.
 	auto &order = sort_order;
 	auto &keys = sort_keys;
-	if (scene_lights)
+	if (scene_lights && !device_lights)
 	{
 		const size_t n = scene_lights->size();
 		// gather_positional_lights (renderer/scene.cpp:333-358): only lights whose world-space AABB
@@ -368,6 +368,8 @@ void LightClusterer::refresh_bindless_prepare(const RenderContext &ctx)
 			shadow_maps.push_back(l.light->get_shadow_map());
 		index++;
 	}
+	if (device_lights)
+		index = (unsigned)std::min<int32_t>(device_lights->list.count, ClustererMaxLightsBindless);
 
 	std::memset(&parameters, 0, sizeof(parameters));
 	parameters.num_lights = (int32_t)index;
@@ -393,6 +395,25 @@ void LightClusterer::refresh_bindless_prepare(const RenderContext &ctx)
 	parameters.z_scale = 1.0f / z_slice_size;
 	parameters.z_max_index = (int32_t)resolution_z - 1;
 
+	if (device_lights)
+	{
+		// the camera terms of the device prep; the per-light work is the clustering pass's
+		std::memset(&device_view, 0, sizeof(device_view));
+		for (int i = 0; i < 3; i++)
+		{
+			device_view.camera_position[i] = rp.camera_position[i];
+			device_view.camera_front[i] = rp.camera_front[i];
+		}
+		const vec4 *planes = ctx.get_visibility_frustum().get_planes();
+		for (int p = 0; p < 6; p++)
+			for (int c = 0; c < 4; c++)
+				device_view.planes[4 * p + c] = planes[p][c];
+		device_view.z_slice_extent = z_slice_size;
+		device_view.z_max_index = (int32_t)resolution_z - 1;
+		device_view.frustum_culling = frustum_culling ? 1 : 0;
+		return;
+	}
+
 	// update_bindless_range_buffer_gpu: per-light slice range on the host
 	volume_index_range.resize(index);
 	for (unsigned i = 0; i < index; i++)
@@ -415,6 +436,23 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 	if (!context || !transforms_buffer)
 	{
 		Vulkan::log_error("LightClusterer: refresh() / setup_render_pass_resources() must run before the clustering pass.\n");
+		return;
+	}
+	if (device_lights)
+	{
+		// the device prep writes this frame's copy of "cluster-transforms" in place of the staging upload
+		auto stream = reinterpret_cast<cudaStream_t>(cmd.get_stream());
+		const DeviceLightSource &src = *device_lights;
+		if (src.ready)
+			Vulkan::cuda_ok(cudaStreamWaitEvent(stream, static_cast<cudaEvent_t>(src.ready), 0), "cudaStreamWaitEvent(lights ready)");
+		const GrbClusterBuffers buf = get_cluster_buffers();
+		cmd.check(grb_light_prep(&src.list, &device_view, const_cast<GrbPositionalLight *>(buf.lights), const_cast<float *>(buf.model),
+		                         const_cast<uint32_t *>(buf.type_mask), const_cast<uint32_t *>(buf.z_ranges), src.count, src.scratch, src.scratch_bytes,
+		                         cmd.get_stream_handle()),
+		          "grb_light_prep");
+		if (src.consumed)
+			Vulkan::cuda_ok(cudaEventRecord(static_cast<cudaEvent_t>(src.consumed), stream), "cudaEventRecord(lights consumed)");
+		launch_cluster_kernels(cmd, src.count, std::max<int32_t>(parameters.num_lights, 1));
 		return;
 	}
 	const unsigned n = (unsigned)parameters.num_lights;
@@ -469,7 +507,12 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 		return;
 	Vulkan::cuda_ok(cudaEventRecord(reinterpret_cast<cudaEvent_t>(staging_events[slot]), stream), "cudaEventRecord(staging)");
 	staging_event_pending[slot] = true;
+	launch_cluster_kernels(cmd, nullptr, (int32_t)volume_index_range.size());
+}
 
+// K1 -> K4 over the packed lights of this frame; device_count: the list was packed on the device (counted K3)
+void LightClusterer::launch_cluster_kernels(Vulkan::CommandBuffer &cmd, const int32_t *device_count, int32_t num_ranges)
+{
 	const auto &rp = context->get_render_parameters();
 	GrbCamera cam = {};
 	std::memcpy(cam.view, rp.view.data(), 64);
@@ -494,12 +537,18 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 		tile_y0 = tiles.y0;
 		tile_y1 = tiles.y1;
 	}
+	auto binning = [&](int32_t y0, int32_t y1) {
+		if (device_count)
+			cmd.check(grb_cluster_binning_rows_counted(&parameters, &buf, device_count, y0, y1, cmd.get_stream_handle()), "grb_cluster_binning_rows_counted");
+		else
+			cmd.check(grb_cluster_binning_rows(&parameters, &buf, y0, y1, cmd.get_stream_handle()), "grb_cluster_binning");
+	};
 	if (!lit_tile_ranges.empty())
 		for (const GrbRows &r : lit_tile_ranges)
-			cmd.check(grb_cluster_binning_rows(&parameters, &buf, r.y0, r.y1, cmd.get_stream_handle()), "grb_cluster_binning");
+			binning(r.y0, r.y1);
 	else
-		cmd.check(grb_cluster_binning_rows(&parameters, &buf, tile_y0, tile_y1, cmd.get_stream_handle()), "grb_cluster_binning");
+		binning(tile_y0, tile_y1);
 	// update_bindless_range_buffer_gpu: K4
-	cmd.check(grb_cluster_z_range(&buf, (int32_t)volume_index_range.size(), cmd.get_stream_handle()), "grb_cluster_z_range");
+	cmd.check(grb_cluster_z_range(&buf, num_ranges, cmd.get_stream_handle()), "grb_cluster_z_range");
 }
 } // namespace Granite

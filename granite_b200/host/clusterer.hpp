@@ -87,6 +87,21 @@ public:
 
 	// The scene's positional lights (replaces the ECS gather in renderer/threaded_scene.cpp:112-153).
 	void set_scene_lights(const PositionalLightList *lights) { scene_lights = lights; }
+	// Lights that live in device memory: while a source is set the scene lights are ignored, refresh() fills only the
+	// parameters (num_lights = min(count, ClustererMaxLightsBindless) slots) and the clustering pass culls, sorts and
+	// packs the list on the device (grb_light_prep) before the four kernels, K3 in its counted form.  The kept count
+	// stays on the device at `count`.  `ready` (a cudaEvent_t or null) is waited on before the first read of the
+	// arrays and `consumed` recorded after the last.  Shadowed lights are not supported with it.
+	struct DeviceLightSource
+	{
+		GrbLightList list = {};
+		void *ready = nullptr, *consumed = nullptr;
+		void *scratch = nullptr; // grb_light_prep_scratch_bytes(list.count) or more
+		size_t scratch_bytes = 0;
+		int32_t *count = nullptr; // device
+	};
+	void set_device_lights(const DeviceLightSource *source) { device_lights = source; }
+	bool has_device_lights() const { return device_lights != nullptr; }
 	// the reference always culls the light list against the camera frustum (scene.cpp:333-358)
 	void set_enable_frustum_culling(bool enable) { frustum_culling = enable; }
 
@@ -116,6 +131,8 @@ public:
 private:
 	const RenderContext *context = nullptr;
 	const PositionalLightList *scene_lights = nullptr;
+	const DeviceLightSource *device_lights = nullptr;
+	GrbLightPrepView device_view = {};
 	bool frustum_culling = true;
 	std::vector<uint8_t> visible;
 	unsigned resolution_x = 64, resolution_y = 32, resolution_z = 16;
@@ -160,6 +177,7 @@ private:
 	uvec2 compute_uint_range(vec2 range) const;
 	void refresh_bindless_prepare(const RenderContext &ctx);
 	void build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd);
+	void launch_cluster_kernels(Vulkan::CommandBuffer &cmd, const int32_t *device_count, int32_t num_ranges);
 	void add_render_passes_bindless(RenderGraph &graph);
 	size_t transforms_offset_model() const;
 	size_t transforms_offset_type_mask() const;

@@ -86,6 +86,13 @@ struct GrbhViewer
 
 	std::vector<std::unique_ptr<PositionalLight>> light_storage;
 	PositionalLightList scene_lights;
+	// the caller's light list in device memory (grbh_viewer_set_lights_device) and the prep's scratch, allocated once
+	// for GRBH_MAX_DEVICE_LIGHTS input lights with the kept count in its first bytes; `device_prep_rendered`: a frame
+	// has packed the bound list since it was bound
+	LightClusterer::DeviceLightSource device_lights;
+	void *light_scratch = nullptr;
+	size_t light_scratch_bytes = 0;
+	bool device_prep_rendered = false;
 	std::vector<mat_affine> scene_decals;
 
 	mat4 projection = mat4(1.0f), view = mat4(1.0f);
@@ -926,6 +933,7 @@ void GrbhViewer::render_frame(const GrbhHostGBuffer *host, double frame_time)
 	pending_upload = nullptr;
 	present_target = nullptr;
 	profiled_frames++;
+	device_prep_rendered = cluster.has_device_lights();
 
 	if (config.timestamps == 1)
 		for (auto &iv : device->collect_time_intervals())
@@ -1004,6 +1012,8 @@ extern "C" void grbh_viewer_destroy(GrbhViewer *viewer)
 	for (auto e : viewer->free_output_events)
 		cudaEventDestroy(e);
 	viewer->graph.reset();
+	if (viewer->light_scratch)
+		cudaFree(viewer->light_scratch);
 	if (viewer->device)
 		Granite::release_smaa_lookup_textures(*viewer->device); // device images: must go before the device does
 	delete viewer;
@@ -1041,6 +1051,8 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 	if (!v || !l || l->count < 0)
 		return fail("grbh_viewer_set_lights: bad arguments");
 	GRBH_TRY
+	v->cluster.set_device_lights(nullptr);
+	v->device_prep_rendered = false;
 	v->light_storage.clear();
 	v->scene_lights.clear();
 	for (int i = 0; i < l->count; i++)
@@ -1070,6 +1082,79 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 		}
 		v->scene_lights.push_back(info);
 	}
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDeviceLights *l)
+{
+	const char *fn = "grbh_viewer_set_lights_device: ";
+	if (!v || !l)
+		return fail(std::string(fn) + "null viewer or light list");
+	if (l->count < 0 || l->count > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(std::string(fn) + "count " + std::to_string(l->count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (v->config.clustered_lights_shadows)
+		return fail(std::string(fn) + "the viewer was created with clustered_lights_shadows; shadowed lights need host lights (grbh_viewer_set_lights)");
+	if (!v->device)
+		return fail(std::string(fn) + "host-only viewer (no CUDA device)");
+	GRBH_TRY
+	cudaSetDevice(v->device->get_device_index());
+	if (l->count > 0)
+	{
+		const struct
+		{
+			const char *name;
+			const void *data;
+			size_t bytes;
+		} arrays[] = { { "color", l->color, 12 }, { "position", l->position, 12 }, { "is_point", l->is_point, 1 },
+			           { "rotation", l->rotation, 36 }, { "inner_cone", l->inner_cone, 4 }, { "outer_cone", l->outer_cone, 4 } };
+		for (const auto &a : arrays)
+		{
+			if (!a.data)
+				return fail(std::string(fn) + "null " + a.name);
+			// the first and the last byte of each array are device memory of the viewer's device
+			const uint8_t *base = static_cast<const uint8_t *>(a.data);
+			for (const uint8_t *p : { base, base + a.bytes * (size_t)l->count - 1 })
+			{
+				cudaPointerAttributes attr = {};
+				const cudaError_t err = cudaPointerGetAttributes(&attr, p);
+				if (err != cudaSuccess)
+					cudaGetLastError();
+				if (err != cudaSuccess || (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) ||
+				    attr.device != v->device->get_device_index())
+					return fail(std::string(fn) + a.name + " is not device memory of the viewer's device (" + std::to_string(v->device->get_device_index()) +
+					            ")");
+			}
+		}
+	}
+	if (!v->light_scratch)
+	{
+		const uint64_t bytes = grb_light_prep_scratch_bytes(GRBH_MAX_DEVICE_LIGHTS);
+		if (bytes == 0)
+			return fail(std::string(fn) + "grb_light_prep_scratch_bytes failed: " + grb_last_error_string());
+		if (!Vulkan::cuda_ok(cudaMalloc(&v->light_scratch, (size_t)bytes + 256), "cudaMalloc(light prep scratch)"))
+		{
+			v->light_scratch = nullptr;
+			return fail(std::string(fn) + "cudaMalloc of the prep scratch failed");
+		}
+		v->light_scratch_bytes = (size_t)bytes;
+	}
+	auto &d = v->device_lights;
+	d.list.count = l->count;
+	d.list.color = l->color;
+	d.list.position = l->position;
+	d.list.is_point = l->is_point;
+	d.list.rotation = l->rotation;
+	d.list.inner_cone = l->inner_cone;
+	d.list.outer_cone = l->outer_cone;
+	d.list.cutoff_range = l->cutoff_range;
+	d.ready = l->ready;
+	d.consumed = l->consumed;
+	d.count = static_cast<int32_t *>(v->light_scratch);
+	d.scratch = static_cast<uint8_t *>(v->light_scratch) + 256;
+	d.scratch_bytes = v->light_scratch_bytes;
+	v->cluster.set_device_lights(&d);
+	v->device_prep_rendered = false;
 	return 0;
 	GRBH_CATCH
 }
@@ -1730,6 +1815,32 @@ extern "C" int32_t grbh_viewer_get_light_prep(GrbhViewer *v, GrbPositionalLight 
 {
 	if (!v)
 		return fail("null viewer");
+	if (v->cluster.has_device_lights())
+	{
+		if (!v->device_prep_rendered)
+			return fail("grbh_viewer_get_light_prep: no frame has been rendered since the device lights were bound");
+		GRBH_TRY
+		cudaSetDevice(v->device->get_device_index());
+		v->device->wait_idle();
+		const GrbClusterBuffers buf = v->cluster.get_cluster_buffers();
+		int32_t n = 0;
+		if (!Vulkan::cuda_ok(cudaMemcpy(&n, v->device_lights.count, sizeof(n), cudaMemcpyDeviceToHost), "cudaMemcpy(count)"))
+			return fail("grbh_viewer_get_light_prep: reading the device count failed");
+		if (n > capacity)
+			return fail("grbh_viewer_get_light_prep: capacity too small");
+		const std::pair<void *, std::pair<const void *, size_t>> copies[] = {
+			{ records, { buf.lights, sizeof(GrbPositionalLight) * (size_t)n } },
+			{ model_rows, { buf.model, 48 * (size_t)n } },
+			{ type_mask, { buf.type_mask, sizeof(uint32_t) * (size_t)((n + 31) / 32) } },
+			{ z_ranges, { buf.z_ranges, sizeof(uint32_t) * 2 * (size_t)std::max(n, 1) } },
+		};
+		for (const auto &c : copies)
+			if (c.first && c.second.second &&
+			    !Vulkan::cuda_ok(cudaMemcpy(c.first, c.second.first, c.second.second, cudaMemcpyDeviceToHost), "cudaMemcpy(light prep)"))
+				return fail("grbh_viewer_get_light_prep: reading the device prep failed");
+		return n;
+		GRBH_CATCH
+	}
 	// host prep only (no GPU work): usable on a machine without a device
 	v->cluster.set_scene_lights(&v->scene_lights);
 	if (v->config.cluster_res[0])

@@ -32,6 +32,15 @@ class GrbhLights(C.Structure):
                 ("rotation", C.c_void_p), ("inner_cone", C.c_void_p), ("outer_cone", C.c_void_p), ("cutoff_range", C.c_float)]
 
 
+class GrbhDeviceLights(C.Structure):
+    _fields_ = [("count", C.c_int32), ("color", C.c_void_p), ("position", C.c_void_p), ("is_point", C.c_void_p),
+                ("rotation", C.c_void_p), ("inner_cone", C.c_void_p), ("outer_cone", C.c_void_p), ("cutoff_range", C.c_float),
+                ("ready", C.c_void_p), ("consumed", C.c_void_p)]
+
+
+MAX_DEVICE_LIGHTS = 65536
+
+
 class GrbhHostGBuffer(C.Structure):
     _fields_ = [("albedo", C.c_void_p), ("normal", C.c_void_p), ("pbr", C.c_void_p), ("depth", C.c_void_p),
                 ("emissive", C.c_void_p), ("mv", C.c_void_p)]
@@ -398,6 +407,37 @@ class Viewer:
         l = GrbhLights(n, _vp(arrs["color"]), _vp(arrs["position"]), _vp(arrs["is_point"]), _vp(arrs["rotation"]),
                        _vp(arrs["inner"]), _vp(arrs["outer"]), cutoff)
         _check(lib().grbh_viewer_set_lights(self._h, C.byref(l)), "grbh_viewer_set_lights")
+
+    def set_lights_device(self, color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, ready=None, consumed=None):
+        """Binds a light list in device memory (grbh_viewer_set_lights_device) from the next frame until the next
+        set_lights[_device] call: torch CUDA tensors on the viewer's device, contiguous, in synth.Lights' shapes --
+        color and position (N, 3) float32, is_point (N,) bool or uint8, rotation (N, 3, 3) float32 column-major,
+        inner_cone and outer_cone (N,) float32.  Every frame culls, sorts and packs them on the GPU, so they may be
+        updated in place between frames.  ready: a torch.cuda.Event each frame's clustering pass waits on before it
+        reads them; consumed: a torch.cuda.Event the viewer records after its last read.  The tensors must stay alive
+        while frames that read them are in flight."""
+        import torch
+
+        n = int(color.shape[0]) if isinstance(color, torch.Tensor) and color.dim() == 2 else -1
+        want = {"color": (color, (n, 3), (torch.float32,)), "position": (position, (n, 3), (torch.float32,)),
+                "is_point": (is_point, (n,), (torch.bool, torch.uint8)), "rotation": (rotation, (n, 3, 3), (torch.float32,)),
+                "inner_cone": (inner_cone, (n,), (torch.float32,)), "outer_cone": (outer_cone, (n,), (torch.float32,))}
+        for name, (t, shape, dtypes) in want.items():
+            if not isinstance(t, torch.Tensor) or not t.is_cuda:
+                raise ValueError(f"set_lights_device: {name} must be a torch CUDA tensor")
+            if tuple(t.shape) != shape or t.dtype not in dtypes:
+                raise ValueError(f"set_lights_device: {name} must be {shape} of {' or '.join(str(d) for d in dtypes)}, got "
+                                 f"{tuple(t.shape)} {t.dtype}")
+            if not t.is_contiguous():
+                raise ValueError(f"set_lights_device: {name} must be contiguous")
+        for ev in (ready, consumed):
+            if ev is not None and not ev.cuda_event:
+                ev.record()  # torch creates the CUDA event on its first record
+        l = GrbhDeviceLights(n, color.data_ptr(), position.data_ptr(), is_point.data_ptr(), rotation.data_ptr(), inner_cone.data_ptr(),
+                             outer_cone.data_ptr(), cutoff, None if ready is None else ready.cuda_event,
+                             None if consumed is None else consumed.cuda_event)
+        _check(lib().grbh_viewer_set_lights_device(self._h, C.byref(l)), "grbh_viewer_set_lights_device")
+        self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone)
 
     def init_collectives(self, unique_id: bytes, rank: int, world: int):
         buf = (C.c_uint8 * 128).from_buffer_copy(unique_id)

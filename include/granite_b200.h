@@ -160,6 +160,51 @@ int32_t grb_cluster_z_range(const GrbClusterBuffers *buf, int32_t num_ranges, vo
 int32_t grb_cluster_build(const GrbCamera *cam, const GrbClusterParameters *params,
                           const GrbClusterBuffers *buf, void *stream);
 
+/* K3 for a light list prepared on the device (grb_light_prep): params->num_lights is the number of SLOTS, the kept
+ * count is read from `device_count` on the device.  Bits of lights >= count are cleared and the words at or past
+ * ceil(count / 32) are written as zero without testing, so a tile's words equal those of a host-prepared list of
+ * `count` lights and are zero after them, whatever the buffer held before.  Rows as grb_cluster_binning_rows. */
+int32_t grb_cluster_binning_rows_counted(const GrbClusterParameters *params, const GrbClusterBuffers *buffers, const int32_t *device_count,
+                                         int32_t tile_y0, int32_t tile_y1, void *stream);
+
+/* ---- light prep on the device: LightClusterer::refresh_bindless_prepare for a light list in device memory ---- */
+#define GRB_MAX_CLUSTER_LIGHTS 4096 /* ClustererMaxLightsBindless */
+/* The raw lights, device arrays in the layout of the host viewer's GrbhLights. */
+typedef struct GrbLightList
+{
+	int32_t count;
+	const float *color;      /* count x 3 */
+	const float *position;   /* count x 3 */
+	const uint8_t *is_point; /* count: 1 point light, 0 spot light */
+	const float *rotation;   /* count x 9, column-major 3x3 (spot lights) */
+	const float *inner_cone; /* count (spot lights) */
+	const float *outer_cone; /* count (spot lights) */
+	float cutoff_range;
+} GrbLightList;
+/* The camera terms of the prep, computed on the host from the frame's camera. */
+typedef struct GrbLightPrepView
+{
+	float camera_position[3];
+	float camera_front[3];
+	float planes[24];      /* the six visibility-frustum planes (x, y, z, w) of Frustum::build_planes */
+	float z_slice_extent;  /* min(0.5, z_far / resolution_z) */
+	int32_t z_max_index;   /* resolution_z - 1 */
+	int32_t frustum_culling;
+} GrbLightPrepView;
+/* Scratch bytes grb_light_prep needs for up to max_lights input lights (sort keys, indices, the radix sort's
+ * temporary storage).  Queries the current device; 0 on an error. */
+uint64_t grb_light_prep_scratch_bytes(int32_t max_lights);
+/* Culls, sorts front to back and packs lights->count lights into the "cluster-transforms" layout of
+ * slots = min(lights->count, GRB_MAX_CLUSTER_LIGHTS): records[slots], model[slots x 12], type_mask[GRB_MAX_CLUSTER_LIGHTS / 32]
+ * and z_ranges[max(slots, 1) x 2].  The visible lights, in ascending dot(position, camera_front) with ties in input
+ * order, fill the first count = min(visible, GRB_MAX_CLUSTER_LIGHTS) slots with the host prep's bytes; slots
+ * [count, slots) get a zero record and model, a zero type bit and the Z range (~0u, 0).  `count` is written to
+ * *device_count and never read back.  Three steps on `stream`: a cull-and-key kernel, CUB's device radix sort, a pack
+ * kernel.  GRB_ERR_INVALID_ARGUMENT: a null pointer, a count outside 0..65536 or scratch smaller than
+ * grb_light_prep_scratch_bytes(lights->count). */
+int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
+                       uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream);
+
 /* Volumetric-decal binning over the clusterer's tile grid: LightClusterer::update_bindless_mask_buffer_decal_gpu
  * (clusterer.cpp:1391-1461) + clusterer_bindless_binning_decal.comp.  mvps: num_decals x mat4 (column-major, device) =
  * view_projection * decal world transform (clusterer.cpp:1406-1410); boxes: scratch, num_decals x 4 floats (the decals'

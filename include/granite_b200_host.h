@@ -86,6 +86,23 @@ typedef struct GrbhLights
 	float cutoff_range;       /* PositionalLight::set_maximum_range */
 } GrbhLights;
 
+/* The same light list in device memory on the viewer's device (grbh_viewer_set_lights_device): the clustering pass culls,
+ * sorts and packs it on the GPU every frame, so lights that a GPU pass moves never go through the host. */
+#define GRBH_MAX_DEVICE_LIGHTS 65536
+typedef struct GrbhDeviceLights
+{
+	int32_t count;            /* 0 .. GRBH_MAX_DEVICE_LIGHTS */
+	const float *color;       /* device, count x 3 */
+	const float *position;    /* device, count x 3 */
+	const uint8_t *is_point;  /* device, count */
+	const float *rotation;    /* device, count x 9, column-major (as GrbhLights) */
+	const float *inner_cone;  /* device, count */
+	const float *outer_cone;  /* device, count */
+	float cutoff_range;
+	void *ready;    /* cudaEvent_t or NULL: the clustering pass waits on it before it reads */
+	void *consumed; /* cudaEvent_t or NULL: recorded right after the prep's last read */
+} GrbhDeviceLights;
+
 /* Host-memory G-buffer of the full frame (pinned memory makes the uploads asynchronous).
  * Only the rows this rank needs (its band + halo) are copied.  mv may be NULL without TAA. */
 typedef struct GrbhHostGBuffer
@@ -122,6 +139,13 @@ void grbh_viewer_destroy(GrbhViewer *viewer);
 int32_t grbh_viewer_set_camera(GrbhViewer *viewer, const float *projection16, const float *view16);
 int32_t grbh_viewer_set_directional(GrbhViewer *viewer, const float *color3, const float *direction3);
 int32_t grbh_viewer_set_lights(GrbhViewer *viewer, const GrbhLights *lights);
+/* Binds a light list in device memory from the next frame until the next grbh_viewer_set_lights[_device] call
+ * (grbh_viewer_set_lights goes back to host lights).  Every frame's clustering pass reads the arrays after `ready`, so
+ * the caller may update them in place between frames; it culls, sorts and packs them on the GPU into the same bytes
+ * the host prep of the same lights gives, and the kept count never comes back to the host.  The arrays must be device
+ * memory of the viewer's device and stay alive while frames that read them are in flight.  Refused: a host-only viewer,
+ * a count outside 0..GRBH_MAX_DEVICE_LIGHTS, a viewer created with clustered_lights_shadows. */
+int32_t grbh_viewer_set_lights_device(GrbhViewer *viewer, const GrbhDeviceLights *lights);
 int32_t grbh_viewer_set_exposure(GrbhViewer *viewer, float exposure);
 /* Shadow maps of the lights of the last grbh_viewer_set_lights call, in THAT order: `count` device pointers (host array),
  * each D16_UNORM of resolution^2 texels (spot) or 6 x resolution^2 (point, faces +X -X +Y -Y +Z -Z); null = no shadow.
@@ -299,7 +323,9 @@ int32_t grbh_viewer_join_streams(GrbhViewer *viewer);
 int32_t grbh_viewer_get_image(GrbhViewer *viewer, const char *resource_name, GrbImage *out);
 int32_t grbh_viewer_get_buffer(GrbhViewer *viewer, const char *resource_name, void **device_ptr, uint64_t *size);
 int32_t grbh_viewer_get_cluster(GrbhViewer *viewer, GrbClusterParameters *params, GrbClusterBuffers *buffers);
-/* Copies the sorted/packed host-side light data of the last refresh (for host-prep parity tests). */
+/* Copies the sorted/packed host-side light data of the last refresh (for host-prep parity tests).  With device lights
+ * bound it copies the device prep of the last rendered frame instead -- the kept count, its records, model rows, type
+ * mask words and Z ranges (one (~0u, 0) range when the count is 0) -- after waiting for the device to go idle. */
 int32_t grbh_viewer_get_light_prep(GrbhViewer *viewer, GrbPositionalLight *records, float *model_rows, uint32_t *type_mask, uint32_t *z_ranges,
                                    int32_t capacity);
 int32_t grbh_viewer_get_camera(GrbhViewer *viewer, GrbCamera *out, float *projection16, float *inv_projection16);

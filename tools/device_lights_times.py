@@ -1,0 +1,139 @@
+#!/usr/bin/env python3
+"""Frames/s of BASELINE config c3 (3840x2160, bloom + tonemap) fed from device G-buffers, with the positional lights
+moved every frame by a small torch op on the device, by where the light prep runs:
+- "host lights": the moved positions are copied to the host and handed over with set_lights every frame, so the
+  clusterer culls, sorts and packs them on the CPU and uploads the result;
+- "device lights": set_lights_device binds the tensors once; every frame's clustering pass culls, sorts and packs them
+  on the GPU.
+
+    python tools/device_lights_times.py [--frames 100]
+    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100]
+
+Two light lists: 4096 input lights (all in view), and 16384 input lights of which 4096 are kept.  Under torchrun, one
+rank per GPU, row-sharded frames with every rank binding its own copy of the lights; the sharded rate is that of the
+slowest rank.
+
+Each viewer renders 4 untimed frames, then --frames timed frames (CUDA events on the viewer's stream), and reports the
+host time spent recording them (the frame calls and the light hand-over, per frame).  The "clustering-bindless" pass
+time comes from a second run of the same frames with the viewer's timestamps on.  The card's name and power limit come
+from a read-only nvidia-smi query in the same run and are printed beside every number.
+"""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from granite_b200 import synth, viewer  # noqa: E402
+from tests import device_lights_cases as cases  # noqa: E402
+from tests import sharded  # noqa: E402
+from tools.device_gbuffer_times import FILL, H, W, device_gbuffers  # noqa: E402
+
+
+def light_list(n):
+    """n lights: the first 4096 in view (synth.make_lights), the rest behind the eye, so at most 4096 are kept."""
+    kept = synth.make_lights(min(n, 4096), spot_fraction=0.0, aspect=W / H)
+    if n <= 4096:
+        return kept
+    extra = synth.make_lights(n - 4096, spot_fraction=0.0, aspect=W / H)
+    extra.position[:, 2] += 400.0
+    return synth.Lights(*[np.concatenate([a, b]) for a, b in zip((kept.color, kept.position, kept.is_point, kept.rot, kept.inner_cone, kept.outer_cone),
+                                                                   (extra.color, extra.position, extra.is_point, extra.rot, extra.inner_cone,
+                                                                    extra.outer_cone))])
+
+
+def timed(v, stream, frames, step):
+    """(ms of `frames` frames of step(v, i) after FILL untimed ones, host ms per frame spent in the step calls)."""
+    for i in range(FILL):
+        step(v, i)
+    v.sync()
+    if torch.distributed.is_initialized():
+        torch.distributed.barrier()
+    a0, a1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    a0.record(stream)
+    t0 = time.perf_counter()
+    for i in range(frames):
+        step(v, FILL + i)
+    host_ms = (time.perf_counter() - t0) * 1e3 / frames
+    v.join_streams()
+    a1.record(stream)
+    torch.cuda.synchronize()
+    return a0.elapsed_time(a1), host_ms
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=100)
+    args = ap.parse_args()
+    distributed = "RANK" in os.environ
+    if distributed:
+        rank, world, local = sharded.init_ranks(allow_shared=False)
+    else:
+        rank, world, local = 0, 1, 0
+        torch.cuda.set_device(0)
+    card = sharded.card(local)
+    scene = synth.make_scene(W, H)
+    dev = device_gbuffers(W, H)
+    bands = viewer.band_partition(H, world) if world > 1 else None
+    result = {"workload": "c3: 3840x2160, bloom + tonemap, device G-buffer every frame, lights moved on the device every frame",
+              "frames_timed": args.frames, "fill_frames": FILL, "ranks": world, "gpu": card, "runs": []}
+
+    for n in (4096, 16384):
+        lights = light_list(n)
+        for mode in ("host lights", "device lights"):
+            def make(extra):
+                return sharded.make_viewer(W, H, scene, lights, scene.view, bands=bands, **extra)
+
+            def stepper():
+                state = {"viewer": None}
+                d = cases.to_device(lights)
+                phase = 0.01 * torch.sin(torch.arange(n, device="cuda", dtype=torch.float32))[:, None]
+
+                def step(v, i):
+                    if state["viewer"] is not v:
+                        state["viewer"] = v
+                        state["gbs"] = [v.device_gbuffer(*g) for g in dev]
+                        if mode == "device lights":
+                            v.set_lights_device(**d)
+                    d["position"].add_(phase)  # the lights' own per-frame update, on the device
+                    if mode == "host lights":
+                        v.set_lights(synth.Lights(lights.color, d["position"].cpu().numpy(), lights.is_point, lights.rot, lights.inner_cone,
+                                                  lights.outer_cone))
+                    v.render_frame_device(state["gbs"][i % 2])
+                return step
+
+            closer = sharded.close_sharded if distributed else (lambda v: v.close())
+            stream = torch.cuda.Stream()
+            v = make(dict(stream=stream.cuda_stream))
+            ms, host_ms = timed(v, stream, args.frames, stepper())
+            kept = v.light_prep()[0]
+            closer(v)
+            stream = torch.cuda.Stream()
+            v = make(dict(stream=stream.cuda_stream, timestamps=True))
+            timed(v, stream, args.frames, stepper())
+            t, c = v.collect_timings().get("clustering-bindless", (0.0, 0))
+            closer(v)
+            run = {"input_lights": n, "kept_lights": kept, "mode": mode, "ms": ms, "host_ms_per_frame": round(host_ms, 4),
+                   "clustering_pass_ms": round(t / max(c, 1), 4), "gpu": card}
+            if distributed:
+                gathered = [None] * world
+                torch.distributed.all_gather_object(gathered, dict(run, rank=rank))
+                run = {"input_lights": n, "mode": mode, "frames_per_s": round(args.frames / (max(g["ms"] for g in gathered) * 1e-3), 2),
+                       "ranks": gathered}
+            else:
+                run["frames_per_s"] = round(args.frames / (ms * 1e-3), 2)
+            result["runs"].append(run)
+    if rank == 0:
+        print(json.dumps(result), flush=True)
+    if distributed:
+        torch.distributed.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()
