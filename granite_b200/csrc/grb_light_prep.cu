@@ -9,11 +9,14 @@
 //   2. cub::DeviceRadixSort::SortPairs over those 33 bits -- stable, so equal keys keep input order, which is the host's
 //      by_key_then_input comparator;
 //   3. pack_kernel, one thread per slot of GRB_MAX_CLUSTER_LIGHTS: the visible count is where the culled keys begin
-//      (a binary search of the sorted keys), and slot s < count packs sorted light s.
+//      (a binary search of the sorted keys), and slot s < count packs sorted light s (grb_light_prep_shadowed: with its
+//      shadow transform and map).
 #include "grb_common.cuh"
 #include "grb_light_prep.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
+
+#include <string>
 
 namespace grb
 {
@@ -34,10 +37,13 @@ __global__ void __launch_bounds__(256) cull_key_kernel(GrbLightList lights, GrbL
 	values[i] = (uint32_t)i;
 }
 
-__global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights, GrbLightPrepView view, const unsigned long long *__restrict__ keys,
-                                                           const uint32_t *__restrict__ order, GrbPositionalLight *__restrict__ records,
-                                                           float *__restrict__ model, uint32_t *__restrict__ type_mask, uint2 *__restrict__ z_ranges,
-                                                           int32_t *__restrict__ count_out)
+// Shadowed: the shadow tables too (lp::pack_shadow); grb_light_prep runs the <false> form, whose code has no shadow part.
+template <bool Shadowed>
+__global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights, GrbLightShadowList shadows, GrbLightPrepView view,
+                                                           const unsigned long long *__restrict__ keys, const uint32_t *__restrict__ order,
+                                                           GrbPositionalLight *__restrict__ records, float *__restrict__ model,
+                                                           uint32_t *__restrict__ type_mask, uint2 *__restrict__ z_ranges, float *__restrict__ shadow_transforms,
+                                                           const void **__restrict__ shadow_maps, int32_t *__restrict__ count_out)
 {
 	__shared__ int s_count;
 	if (threadIdx.x == 0)
@@ -59,6 +65,8 @@ __global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights,
 	const int slots = min(lights.count, GRB_MAX_CLUSTER_LIGHTS);
 	const int s = blockIdx.x * blockDim.x + threadIdx.x;
 	bool point = false;
+	if (Shadowed && s < slots)
+		lp::pack_shadow(shadows, s < count ? (int)order[s] : -1, s, shadow_transforms, shadow_maps);
 	if (s < count)
 	{
 		const lp::Light L = lp::load_light(lights, (int)order[s]);
@@ -128,23 +136,38 @@ extern "C" uint64_t grb_light_prep_scratch_bytes(int32_t max_lights)
 	return l.total;
 }
 
-extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
-                                  uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+namespace
+{
+// grb_light_prep and grb_light_prep_shadowed: the checks of grb_light_prep, then the three steps; shadows null = the
+// unshadowed pack kernel
+int32_t light_prep(const char *fn, const GrbLightList *lights, const GrbLightShadowList *shadows, const GrbLightPrepView *view,
+                   GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms,
+                   const void **shadow_maps, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
 {
 	if (!lights || !view || !records || !model || !type_mask || !z_ranges || !device_count || lights->count < 0 || lights->count > kMaxInputLights ||
 	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone ||
 	                           !lights->outer_cone || !scratch)))
 	{
-		set_last_error("grb_light_prep: a null pointer or a count outside 0..65536");
+		set_last_error((std::string(fn) + ": a null pointer or a count outside 0..65536").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (shadows && (!shadow_transforms || !shadow_maps || (lights->count > 0 && (!shadows->transforms || !shadows->maps))))
+	{
+		set_last_error((std::string(fn) + ": a null shadow table").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (shadows && (((uintptr_t)shadow_transforms & 7) || ((uintptr_t)shadows->maps & 7) || ((uintptr_t)shadow_maps & 7)))
+	{
+		set_last_error((std::string(fn) + ": the output transforms, the map array or the output maps are not 8-byte aligned").c_str());
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	const int n = lights->count;
 	ScratchLayout l;
 	if (!scratch_layout(n, l))
-		return check_launch("grb_light_prep: radix sort size");
+		return check_launch((std::string(fn) + ": radix sort size").c_str());
 	if (scratch_bytes < l.total)
 	{
-		set_last_error("grb_light_prep: scratch smaller than grb_light_prep_scratch_bytes(count)");
+		set_last_error((std::string(fn) + ": scratch smaller than grb_light_prep_scratch_bytes(count)").c_str());
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	auto *base = static_cast<uint8_t *>(scratch);
@@ -154,14 +177,40 @@ extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrep
 	if (n > 0)
 	{
 		cull_key_kernel<<<(n + 255) / 256, 256, 0, s>>>(*lights, *view, keys_in, values_in);
-		int32_t r = check_launch("grb_light_prep: cull");
+		int32_t r = check_launch((std::string(fn) + ": cull").c_str());
 		if (r != GRB_OK)
 			return r;
 		size_t temp_bytes = l.temp_bytes;
 		if (cub::DeviceRadixSort::SortPairs(base + l.temp, temp_bytes, keys_in, keys_out, values_in, values_out, n, 0, 33, s) != cudaSuccess)
-			return check_launch("grb_light_prep: sort");
+			return check_launch((std::string(fn) + ": sort").c_str());
 	}
-	pack_kernel<<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, *view, keys_out, values_out, records, model, type_mask,
-	                                                                              reinterpret_cast<uint2 *>(z_ranges), device_count);
-	return check_launch("grb_light_prep: pack");
+	auto *ranges = reinterpret_cast<uint2 *>(z_ranges);
+	if (shadows)
+		pack_kernel<true><<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, *shadows, *view, keys_out, values_out, records, model,
+		                                                                                type_mask, ranges, shadow_transforms, shadow_maps, device_count);
+	else
+		pack_kernel<false><<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, GrbLightShadowList{}, *view, keys_out, values_out, records,
+		                                                                                 model, type_mask, ranges, nullptr, nullptr, device_count);
+	return check_launch((std::string(fn) + ": pack").c_str());
+}
+} // namespace
+
+extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
+                                  uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+{
+	return light_prep("grb_light_prep", lights, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count, scratch,
+	                  scratch_bytes, stream);
+}
+
+extern "C" int32_t grb_light_prep_shadowed(const GrbLightList *lights, const GrbLightShadowList *shadows, const GrbLightPrepView *view,
+                                           GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms_out,
+                                           const void **shadow_maps_out, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+{
+	if (!shadows)
+	{
+		set_last_error("grb_light_prep_shadowed: a null shadow table");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return light_prep("grb_light_prep_shadowed", lights, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out, shadow_maps_out,
+	                  device_count, scratch, scratch_bytes, stream);
 }

@@ -275,5 +275,26 @@ __host__ __device__ inline void pack(const Light &L, const GrbLightPrepView &vie
 	const uint32_t uy = (uint32_t)(int64_t)y;
 	zr[1] = uy < (uint32_t)view.z_max_index ? uy : (uint32_t)view.z_max_index;
 }
+
+// The shadow tables of slot s < slots: the transform and map of input light `src` (>= 0), or a zero matrix and a null
+// map (src < 0).  The input transform is read one float at a time (it may be only 4-byte aligned); the output starts at
+// packed_size(slots) of "cluster-transforms", 8-byte aligned for odd slot counts, so it is stored as float2.
+__host__ __device__ inline void pack_shadow(const GrbLightShadowList &shadows, int src, int s, float *transforms_out, const void **maps_out)
+{
+	float2 *t = reinterpret_cast<float2 *>(transforms_out + 16 * (size_t)s);
+	if (src >= 0)
+	{
+		const float *m = shadows.transforms + 16 * (size_t)src;
+		for (int k = 0; k < 8; k++)
+			t[k] = make_float2(m[2 * k], m[2 * k + 1]);
+		maps_out[s] = shadows.maps[src];
+	}
+	else
+	{
+		for (int k = 0; k < 8; k++)
+			t[k] = make_float2(0.0f, 0.0f);
+		maps_out[s] = nullptr;
+	}
+}
 } // namespace lp
 } // namespace grb

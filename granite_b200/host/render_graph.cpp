@@ -172,7 +172,7 @@ Vulkan::Event RenderPassExternalLockInterface::external_acquire_event()
 	return produced;
 }
 
-void RenderPassExternalLockInterface::external_release_event(Vulkan::Event event)
+void RenderPassExternalLockInterface::external_release_event(Vulkan::Event event, Vulkan::Stream)
 {
 	if (!event)
 		return;
@@ -705,7 +705,7 @@ void RenderGraph::enqueue_render_passes(Vulkan::Device &dev, TaskComposer &compo
 			pass_done_events[p][slot] = dev.request_event();
 		dev.record_event_on(pass_done_events[p][slot], stream);
 		for (auto &l : pass.get_lock_interfaces())
-			l.iface->external_release_event(pass_done_events[p][slot]);
+			l.iface->external_release_event(pass_done_events[p][slot], stream);
 		for (auto *r : pass.get_all_reads())
 			mark(physical_key(*r, false), false);
 		for (auto *w : pass.get_all_writes())

@@ -158,9 +158,11 @@ public:
 	virtual ~RenderPassExternalLockInterface() = default;
 	virtual const char *get_ident() const { return "external-lock"; }
 
-	// consumer side (called by the graph while it records a pass)
-	Vulkan::Event external_acquire_event();
-	void external_release_event(Vulkan::Event event);
+	// consumer side (called by the graph while it records a pass): the pass's stream waits on the acquire event before
+	// the pass, and the release hook gets the event recorded behind the pass and the pass's stream.  An owner whose
+	// writes are not on the graph's device (the caller of the viewer) overrides both with its own events.
+	virtual Vulkan::Event external_acquire_event();
+	virtual void external_release_event(Vulkan::Event event, Vulkan::Stream stream);
 	// External accesses are read-only; the reference records which queues touch the resource, the stream order
 	// plus the two calls above make that unnecessary here.  Kept so that builder code compiles unchanged.
 	void mark_access_in_queue(RenderGraphQueueFlagBits, VkPipelineStageFlags2, VkAccessFlags2) { foreign_access = true; }

@@ -42,6 +42,21 @@ struct FixedExposure : HDRDynamicExposureInterface
 	float exposure = 1.0f;
 	float get_exposure() const override { return exposure; }
 };
+
+// The "bindless-shadowmaps" lock of a shadowed viewer (clusterer.cpp's external lock on the lighting pass): the caller
+// renders the maps of device lights on its own streams, so the lighting pass waits on the caller's `ready` and records
+// the caller's `consumed` behind its last read.  Both null (host lights, or no events given): no CUDA call at all.
+struct ShadowMapEvents : RenderPassExternalLockInterface
+{
+	cudaEvent_t ready = nullptr, consumed = nullptr;
+	const char *get_ident() const override { return "bindless-shadowmaps"; }
+	Vulkan::Event external_acquire_event() override { return ready; }
+	void external_release_event(Vulkan::Event, Vulkan::Stream stream) override
+	{
+		if (consumed)
+			Vulkan::cuda_ok(cudaEventRecord(consumed, stream), "cudaEventRecord(shadow maps consumed)");
+	}
+};
 } // namespace
 
 struct GrbhViewer
@@ -90,6 +105,7 @@ struct GrbhViewer
 	// for GRBH_MAX_DEVICE_LIGHTS input lights with the kept count in its first bytes; `device_prep_rendered`: a frame
 	// has packed the bound list since it was bound
 	LightClusterer::DeviceLightSource device_lights;
+	ShadowMapEvents shadow_map_events;
 	void *light_scratch = nullptr;
 	size_t light_scratch_bytes = 0;
 	bool device_prep_rendered = false;
@@ -303,6 +319,8 @@ void GrbhViewer::bake_render_graph()
 	cluster.set_enable_volumetric_decals(config.volumetric_decals != 0);
 	cluster.set_scene_decals(&scene_decals);
 	cluster.set_enable_shadows(config.clustered_lights_shadows != 0);
+	if (config.clustered_lights_shadows)
+		graph.add_external_lock_interface("bindless-shadowmaps", &shadow_map_events);
 	cluster.set_shadow_resolution(config.clustered_lights_shadow_resolution > 0 ? (unsigned)config.clustered_lights_shadow_resolution : 512u);
 	if (bands.size() > 1)
 	{
@@ -1053,6 +1071,8 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 	GRBH_TRY
 	v->cluster.set_device_lights(nullptr);
 	v->device_prep_rendered = false;
+	v->device_lights.shadows = {};
+	v->shadow_map_events.ready = v->shadow_map_events.consumed = nullptr;
 	v->light_storage.clear();
 	v->scene_lights.clear();
 	for (int i = 0; i < l->count; i++)
@@ -1086,18 +1106,31 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 	GRBH_CATCH
 }
 
-extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDeviceLights *l)
+namespace
 {
-	const char *fn = "grbh_viewer_set_lights_device: ";
-	if (!v || !l)
-		return fail(std::string(fn) + "null viewer or light list");
-	if (l->count < 0 || l->count > GRBH_MAX_DEVICE_LIGHTS)
-		return fail(std::string(fn) + "count " + std::to_string(l->count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
-	if (v->config.clustered_lights_shadows)
-		return fail(std::string(fn) + "the viewer was created with clustered_lights_shadows; shadowed lights need host lights (grbh_viewer_set_lights)");
-	if (!v->device)
-		return fail(std::string(fn) + "host-only viewer (no CUDA device)");
-	GRBH_TRY
+// false (and the error set) unless [data, data + bytes) starts and ends in device memory of the viewer's device
+bool is_viewer_device_memory(GrbhViewer *v, const std::string &fn, const char *name, const void *data, size_t bytes)
+{
+	const uint8_t *base = static_cast<const uint8_t *>(data);
+	for (const uint8_t *p : { base, base + bytes - 1 })
+	{
+		cudaPointerAttributes attr = {};
+		const cudaError_t err = cudaPointerGetAttributes(&attr, p);
+		if (err != cudaSuccess)
+			cudaGetLastError();
+		if (err != cudaSuccess || (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) ||
+		    attr.device != v->device->get_device_index())
+		{
+			fail(fn + name + " is not device memory of the viewer's device (" + std::to_string(v->device->get_device_index()) + ")");
+			return false;
+		}
+	}
+	return true;
+}
+
+// grbh_viewer_set_lights_device[_shadowed] once the arguments that need no CUDA call have passed
+int32_t bind_device_lights(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhDeviceLightShadows *sh, const std::string &fn)
+{
 	cudaSetDevice(v->device->get_device_index());
 	if (l->count > 0)
 	{
@@ -1111,31 +1144,24 @@ extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDevice
 		for (const auto &a : arrays)
 		{
 			if (!a.data)
-				return fail(std::string(fn) + "null " + a.name);
+				return fail(fn + "null " + a.name);
 			// the first and the last byte of each array are device memory of the viewer's device
-			const uint8_t *base = static_cast<const uint8_t *>(a.data);
-			for (const uint8_t *p : { base, base + a.bytes * (size_t)l->count - 1 })
-			{
-				cudaPointerAttributes attr = {};
-				const cudaError_t err = cudaPointerGetAttributes(&attr, p);
-				if (err != cudaSuccess)
-					cudaGetLastError();
-				if (err != cudaSuccess || (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged) ||
-				    attr.device != v->device->get_device_index())
-					return fail(std::string(fn) + a.name + " is not device memory of the viewer's device (" + std::to_string(v->device->get_device_index()) +
-					            ")");
-			}
+			if (!is_viewer_device_memory(v, fn, a.name, a.data, a.bytes * (size_t)l->count))
+				return -1;
 		}
+		if (sh && (!is_viewer_device_memory(v, fn, "shadow transforms", sh->transforms, 64 * (size_t)l->count) ||
+		           !is_viewer_device_memory(v, fn, "shadow maps", sh->maps, 8 * (size_t)l->count)))
+			return -1;
 	}
 	if (!v->light_scratch)
 	{
 		const uint64_t bytes = grb_light_prep_scratch_bytes(GRBH_MAX_DEVICE_LIGHTS);
 		if (bytes == 0)
-			return fail(std::string(fn) + "grb_light_prep_scratch_bytes failed: " + grb_last_error_string());
+			return fail(fn + "grb_light_prep_scratch_bytes failed: " + grb_last_error_string());
 		if (!Vulkan::cuda_ok(cudaMalloc(&v->light_scratch, (size_t)bytes + 256), "cudaMalloc(light prep scratch)"))
 		{
 			v->light_scratch = nullptr;
-			return fail(std::string(fn) + "cudaMalloc of the prep scratch failed");
+			return fail(fn + "cudaMalloc of the prep scratch failed");
 		}
 		v->light_scratch_bytes = (size_t)bytes;
 	}
@@ -1148,14 +1174,53 @@ extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDevice
 	d.list.inner_cone = l->inner_cone;
 	d.list.outer_cone = l->outer_cone;
 	d.list.cutoff_range = l->cutoff_range;
+	d.shadows.transforms = sh ? sh->transforms : nullptr;
+	d.shadows.maps = sh ? reinterpret_cast<const void *const *>(sh->maps) : nullptr;
 	d.ready = l->ready;
 	d.consumed = l->consumed;
 	d.count = static_cast<int32_t *>(v->light_scratch);
 	d.scratch = static_cast<uint8_t *>(v->light_scratch) + 256;
 	d.scratch_bytes = v->light_scratch_bytes;
+	v->shadow_map_events.ready = sh ? static_cast<cudaEvent_t>(sh->maps_ready) : nullptr;
+	v->shadow_map_events.consumed = sh ? static_cast<cudaEvent_t>(sh->maps_consumed) : nullptr;
 	v->cluster.set_device_lights(&d);
 	v->device_prep_rendered = false;
 	return 0;
+}
+} // namespace
+
+extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDeviceLights *l)
+{
+	const std::string fn = "grbh_viewer_set_lights_device: ";
+	if (!v || !l)
+		return fail(fn + "null viewer or light list");
+	if (l->count < 0 || l->count > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(fn + "count " + std::to_string(l->count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (v->config.clustered_lights_shadows)
+		return fail(fn + "the viewer was created with clustered_lights_shadows; its device lights need their shadows "
+		                 "(grbh_viewer_set_lights_device_shadowed)");
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	GRBH_TRY
+	return bind_device_lights(v, l, nullptr, fn);
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhDeviceLightShadows *shadows)
+{
+	const std::string fn = "grbh_viewer_set_lights_device_shadowed: ";
+	if (!v || !l || !shadows)
+		return fail(fn + "null viewer, light list or shadow list");
+	if (l->count < 0 || l->count > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(fn + "count " + std::to_string(l->count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (!v->config.clustered_lights_shadows)
+		return fail(fn + "the viewer was created without clustered_lights_shadows (grbh_viewer_set_lights_device)");
+	if (l->count > 0 && (!shadows->transforms || !shadows->maps))
+		return fail(fn + "null shadow transforms or shadow maps table");
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	GRBH_TRY
+	return bind_device_lights(v, l, shadows, fn);
 	GRBH_CATCH
 }
 
@@ -1858,6 +1923,49 @@ extern "C" int32_t grbh_viewer_get_light_prep(GrbhViewer *v, GrbPositionalLight 
 	if (z_ranges)
 		std::memcpy(z_ranges, v->cluster.get_z_ranges().data(), sizeof(uint32_t) * 2 * v->cluster.get_z_ranges().size());
 	return n;
+}
+
+extern "C" int32_t grbh_viewer_get_light_shadow_prep(GrbhViewer *v, float *transforms16, uint64_t *maps, int32_t capacity)
+{
+	if (!v)
+		return fail("null viewer");
+	if (v->cluster.has_device_lights())
+	{
+		if (!v->config.clustered_lights_shadows)
+			return fail("grbh_viewer_get_light_shadow_prep: the viewer was created without clustered_lights_shadows");
+		if (!v->device_prep_rendered)
+			return fail("grbh_viewer_get_light_shadow_prep: no frame has been rendered since the device lights were bound");
+		GRBH_TRY
+		cudaSetDevice(v->device->get_device_index());
+		v->device->wait_idle();
+		const GrbLightShadows sh = v->cluster.get_light_shadows();
+		int32_t n = 0;
+		if (!Vulkan::cuda_ok(cudaMemcpy(&n, v->device_lights.count, sizeof(n), cudaMemcpyDeviceToHost), "cudaMemcpy(count)"))
+			return fail("grbh_viewer_get_light_shadow_prep: reading the device count failed");
+		if (n > capacity)
+			return fail("grbh_viewer_get_light_shadow_prep: capacity too small");
+		if (n && ((transforms16 && !Vulkan::cuda_ok(cudaMemcpy(transforms16, sh.transforms, 64 * (size_t)n, cudaMemcpyDeviceToHost), "cudaMemcpy(shadow transforms)")) ||
+		          (maps && !Vulkan::cuda_ok(cudaMemcpy(maps, sh.maps, 8 * (size_t)n, cudaMemcpyDeviceToHost), "cudaMemcpy(shadow maps)"))))
+			return fail("grbh_viewer_get_light_shadow_prep: reading the device prep failed");
+		return n;
+		GRBH_CATCH
+	}
+	// host prep only (no GPU work), like grbh_viewer_get_shadow_transforms
+	GRBH_TRY
+	v->cluster.set_scene_lights(&v->scene_lights);
+	v->cluster.set_enable_shadows(true);
+	v->cluster.refresh(v->context);
+	v->cluster.set_enable_shadows(v->config.clustered_lights_shadows != 0);
+	const auto &t = v->cluster.get_shadow_transforms();
+	const auto &m = v->cluster.get_shadow_maps();
+	if ((int64_t)t.size() > capacity)
+		return fail("grbh_viewer_get_light_shadow_prep: capacity too small");
+	if (transforms16 && !t.empty())
+		std::memcpy(transforms16, t.data(), 64 * t.size());
+	for (size_t i = 0; maps && i < m.size(); i++)
+		maps[i] = (uint64_t)(uintptr_t)m[i];
+	return (int32_t)t.size();
+	GRBH_CATCH
 }
 
 extern "C" int32_t grbh_viewer_set_decals(GrbhViewer *v, const float *world_rows12, int32_t count)

@@ -38,6 +38,10 @@ class GrbhDeviceLights(C.Structure):
                 ("ready", C.c_void_p), ("consumed", C.c_void_p)]
 
 
+class GrbhDeviceLightShadows(C.Structure):
+    _fields_ = [("transforms", C.c_void_p), ("maps", C.c_void_p), ("maps_ready", C.c_void_p), ("maps_consumed", C.c_void_p)]
+
+
 MAX_DEVICE_LIGHTS = 65536
 
 
@@ -408,36 +412,57 @@ class Viewer:
                        _vp(arrs["inner"]), _vp(arrs["outer"]), cutoff)
         _check(lib().grbh_viewer_set_lights(self._h, C.byref(l)), "grbh_viewer_set_lights")
 
-    def set_lights_device(self, color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, ready=None, consumed=None):
+    def set_lights_device(self, color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, ready=None, consumed=None,
+                          shadow_transforms=None, shadow_maps=None, maps_ready=None, maps_consumed=None):
         """Binds a light list in device memory (grbh_viewer_set_lights_device) from the next frame until the next
         set_lights[_device] call: torch CUDA tensors on the viewer's device, contiguous, in synth.Lights' shapes --
         color and position (N, 3) float32, is_point (N,) bool or uint8, rotation (N, 3, 3) float32 column-major,
         inner_cone and outer_cone (N,) float32.  Every frame culls, sorts and packs them on the GPU, so they may be
         updated in place between frames.  ready: a torch.cuda.Event each frame's clustering pass waits on before it
         reads them; consumed: a torch.cuda.Event the viewer records after its last read.  The tensors must stay alive
-        while frames that read them are in flight."""
+        while frames that read them are in flight.
+
+        A viewer created with light_shadows takes each light's shadow too (grbh_viewer_set_lights_device_shadowed), in
+        the same order: shadow_transforms (N, 16) or (N, 4, 4) float32, column-major, the matrix the light's map was
+        rendered with; shadow_maps (N,) int64 of map data_ptr()s, 0 = no shadow.  Both are read with the lights, under
+        ready / consumed.  maps_ready: a torch.cuda.Event the lighting pass waits on before it samples the maps;
+        maps_consumed: one the viewer records behind the lighting pass's last read of them."""
         import torch
 
+        shadowed = shadow_transforms is not None or shadow_maps is not None
         n = int(color.shape[0]) if isinstance(color, torch.Tensor) and color.dim() == 2 else -1
-        want = {"color": (color, (n, 3), (torch.float32,)), "position": (position, (n, 3), (torch.float32,)),
-                "is_point": (is_point, (n,), (torch.bool, torch.uint8)), "rotation": (rotation, (n, 3, 3), (torch.float32,)),
-                "inner_cone": (inner_cone, (n,), (torch.float32,)), "outer_cone": (outer_cone, (n,), (torch.float32,))}
-        for name, (t, shape, dtypes) in want.items():
+        want = {"color": (color, [(n, 3)], (torch.float32,)), "position": (position, [(n, 3)], (torch.float32,)),
+                "is_point": (is_point, [(n,)], (torch.bool, torch.uint8)), "rotation": (rotation, [(n, 3, 3)], (torch.float32,)),
+                "inner_cone": (inner_cone, [(n,)], (torch.float32,)), "outer_cone": (outer_cone, [(n,)], (torch.float32,))}
+        if shadowed:
+            want["shadow_transforms"] = (shadow_transforms, [(n, 16), (n, 4, 4)], (torch.float32,))
+            want["shadow_maps"] = (shadow_maps, [(n,)], (torch.int64,))
+        for name, (t, shapes, dtypes) in want.items():
             if not isinstance(t, torch.Tensor) or not t.is_cuda:
                 raise ValueError(f"set_lights_device: {name} must be a torch CUDA tensor")
-            if tuple(t.shape) != shape or t.dtype not in dtypes:
-                raise ValueError(f"set_lights_device: {name} must be {shape} of {' or '.join(str(d) for d in dtypes)}, got "
-                                 f"{tuple(t.shape)} {t.dtype}")
+            if tuple(t.shape) not in shapes or t.dtype not in dtypes:
+                raise ValueError(f"set_lights_device: {name} must be {' or '.join(str(x) for x in shapes)} of "
+                                 f"{' or '.join(str(d) for d in dtypes)}, got {tuple(t.shape)} {t.dtype}")
             if not t.is_contiguous():
                 raise ValueError(f"set_lights_device: {name} must be contiguous")
-        for ev in (ready, consumed):
+        if not shadowed and (maps_ready is not None or maps_consumed is not None):
+            raise ValueError("set_lights_device: maps_ready / maps_consumed need shadow_transforms and shadow_maps")
+        for ev in (ready, consumed, maps_ready, maps_consumed):
             if ev is not None and not ev.cuda_event:
                 ev.record()  # torch creates the CUDA event on its first record
+
+        def ev(e):
+            return None if e is None else e.cuda_event
+
         l = GrbhDeviceLights(n, color.data_ptr(), position.data_ptr(), is_point.data_ptr(), rotation.data_ptr(), inner_cone.data_ptr(),
-                             outer_cone.data_ptr(), cutoff, None if ready is None else ready.cuda_event,
-                             None if consumed is None else consumed.cuda_event)
-        _check(lib().grbh_viewer_set_lights_device(self._h, C.byref(l)), "grbh_viewer_set_lights_device")
-        self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone)
+                             outer_cone.data_ptr(), cutoff, ev(ready), ev(consumed))
+        if shadowed:
+            sh = GrbhDeviceLightShadows(shadow_transforms.data_ptr(), shadow_maps.data_ptr(), ev(maps_ready), ev(maps_consumed))
+            _check(lib().grbh_viewer_set_lights_device_shadowed(self._h, C.byref(l), C.byref(sh)), "grbh_viewer_set_lights_device_shadowed")
+            self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone, shadow_transforms, shadow_maps)
+        else:
+            _check(lib().grbh_viewer_set_lights_device(self._h, C.byref(l)), "grbh_viewer_set_lights_device")
+            self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone)
 
     def init_collectives(self, unique_id: bytes, rank: int, world: int):
         buf = (C.c_uint8 * 128).from_buffer_copy(unique_id)
@@ -616,6 +641,14 @@ class Viewer:
         zr = np.zeros((capacity + 1, 2), np.uint32)
         n = _check(lib().grbh_viewer_get_light_prep(self._h, _vp(recs), _vp(model), _vp(tmask), _vp(zr), capacity), "grbh_viewer_get_light_prep")
         return n, recs[:n], model[:n], tmask[: (n + 31) // 32], zr[: max(n, 1)]
+
+    def light_shadow_prep(self, capacity=4096):
+        """(transforms (n, 16) float32, maps (n,) uint64) of the light prep in cluster order: the host prep's with host
+        lights, the last frame's device prep with device lights (grbh_viewer_get_light_shadow_prep)."""
+        t = np.zeros((capacity, 16), np.float32)
+        m = np.zeros(capacity, np.uint64)
+        n = _check(lib().grbh_viewer_get_light_shadow_prep(self._h, _vp(t), _vp(m), capacity), "grbh_viewer_get_light_shadow_prep")
+        return t[:n].copy(), m[:n].copy()
 
     def camera(self):
         cam = capi.GrbCamera()

@@ -204,6 +204,22 @@ uint64_t grb_light_prep_scratch_bytes(int32_t max_lights);
  * grb_light_prep_scratch_bytes(lights->count). */
 int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
                        uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream);
+/* The shadows of the lights of a GrbLightList, in the same input order: what the caller rendered each light's map with
+ * and the map itself (GrbLightShadows describes both).  No alignment beyond the element's is assumed of `transforms`. */
+typedef struct GrbLightShadowList
+{
+	const float *transforms;  /* count x 16, column-major, device */
+	const void *const *maps;  /* count device pointers (8-byte aligned array), device; null = no shadow */
+} GrbLightShadowList;
+/* grb_light_prep, plus the shadow tables of the "cluster-transforms" layout: slot s < count gets the transform and the
+ * map pointer of the input light packed into slot s, slots [count, slots) a zero matrix and a null map.
+ * shadow_transforms_out: slots x 16 floats, 8-byte aligned; shadow_maps_out: slots pointers.  The other outputs are
+ * grb_light_prep's bytes.  Same launches as grb_light_prep: the pack kernel writes the tables.
+ * GRB_ERR_INVALID_ARGUMENT: what grb_light_prep refuses, a null table or output, an output transform table that is not
+ * 8-byte aligned, a map array that is not 8-byte aligned. */
+int32_t grb_light_prep_shadowed(const GrbLightList *lights, const GrbLightShadowList *shadows, const GrbLightPrepView *view,
+                                GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms_out,
+                                const void **shadow_maps_out, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream);
 
 /* Volumetric-decal binning over the clusterer's tile grid: LightClusterer::update_bindless_mask_buffer_decal_gpu
  * (clusterer.cpp:1391-1461) + clusterer_bindless_binning_decal.comp.  mvps: num_decals x mat4 (column-major, device) =

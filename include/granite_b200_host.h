@@ -103,6 +103,17 @@ typedef struct GrbhDeviceLights
 	void *consumed; /* cudaEvent_t or NULL: recorded right after the prep's last read */
 } GrbhDeviceLights;
 
+/* The shadows of a device light list (grbh_viewer_set_lights_device_shadowed), in the lights' input order.  The viewer
+ * never computes a shadow transform for device lights: each is the matrix the caller rendered that light's map with
+ * (INTEGRATION.md gives the reference's shadow cameras). */
+typedef struct GrbhDeviceLightShadows
+{
+	const float *transforms; /* device, count x 16, column-major: what GrbLightShadows::transforms holds per light */
+	const uint64_t *maps;    /* device, count map pointers (0 = no shadow), as grbh_viewer_set_light_shadow_maps takes */
+	void *maps_ready;        /* cudaEvent_t or NULL: the lighting pass waits on it before it samples the maps */
+	void *maps_consumed;     /* cudaEvent_t or NULL: recorded on the lighting pass's stream behind its last read of the maps */
+} GrbhDeviceLightShadows;
+
 /* Host-memory G-buffer of the full frame (pinned memory makes the uploads asynchronous).
  * Only the rows this rank needs (its band + halo) are copied.  mv may be NULL without TAA. */
 typedef struct GrbhHostGBuffer
@@ -144,8 +155,16 @@ int32_t grbh_viewer_set_lights(GrbhViewer *viewer, const GrbhLights *lights);
  * the caller may update them in place between frames; it culls, sorts and packs them on the GPU into the same bytes
  * the host prep of the same lights gives, and the kept count never comes back to the host.  The arrays must be device
  * memory of the viewer's device and stay alive while frames that read them are in flight.  Refused: a host-only viewer,
- * a count outside 0..GRBH_MAX_DEVICE_LIGHTS, a viewer created with clustered_lights_shadows. */
+ * a count outside 0..GRBH_MAX_DEVICE_LIGHTS, a viewer created with clustered_lights_shadows (whose device lights go
+ * through grbh_viewer_set_lights_device_shadowed). */
 int32_t grbh_viewer_set_lights_device(GrbhViewer *viewer, const GrbhDeviceLights *lights);
+/* grbh_viewer_set_lights_device for a viewer created with clustered_lights_shadows: the clustering pass also moves each
+ * kept light's shadow transform and map pointer into cluster order, so frames equal those of host lights given the same
+ * maps.  The tables are read by the clustering pass under the lights' ready / consumed events; the maps' texels by the
+ * lighting pass under maps_ready / maps_consumed.  Refused: a null argument, a count outside 0..GRBH_MAX_DEVICE_LIGHTS,
+ * a viewer created without clustered_lights_shadows, null tables with count > 0, a host-only viewer, arrays or tables
+ * that are not device memory of the viewer's device. */
+int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *viewer, const GrbhDeviceLights *lights, const GrbhDeviceLightShadows *shadows);
 int32_t grbh_viewer_set_exposure(GrbhViewer *viewer, float exposure);
 /* Shadow maps of the lights of the last grbh_viewer_set_lights call, in THAT order: `count` device pointers (host array),
  * each D16_UNORM of resolution^2 texels (spot) or 6 x resolution^2 (point, faces +X -X +Y -Y +Z -Z); null = no shadow.
@@ -154,6 +173,10 @@ int32_t grbh_viewer_set_light_shadow_maps(GrbhViewer *viewer, const void *const 
 /* ClustererBindlessTransforms::shadow[i] of the visible lights in cluster order, as the clusterer uploads them (host
  * preparation only, no GPU work): capacity x 16 floats.  Returns the light count. */
 int32_t grbh_viewer_get_shadow_transforms(GrbhViewer *viewer, float *out16_per_light, int32_t capacity);
+/* The shadow tables of the light prep in cluster order (for parity tests): capacity x 16 floats and capacity map pointers
+ * (either may be NULL).  Host lights: the host prep's, no GPU work.  Device lights: the last rendered frame's device prep,
+ * after waiting for the device to go idle, as grbh_viewer_get_light_prep.  Returns the kept light count. */
+int32_t grbh_viewer_get_light_shadow_prep(GrbhViewer *viewer, float *transforms16, uint64_t *maps, int32_t capacity);
 
 /* The two lookup textures SMAA samples (the payloads of the reference's assets/textures/smaa/area.gtx: 160x560 R8G8_UNORM,
  * and search.gtx: 64x16 R8_UNORM), uploaded once to the viewer's device.  grbh_load_gtx reads such a container from a

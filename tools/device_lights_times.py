@@ -6,8 +6,13 @@ moved every frame by a small torch op on the device, by where the light prep run
 - "device lights": set_lights_device binds the tensors once; every frame's clustering pass culls, sorts and packs them
   on the GPU.
 
-    python tools/device_lights_times.py [--frames 100]
-    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100]
+    python tools/device_lights_times.py [--frames 100] [--shadows]
+    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows]
+
+--shadows: viewers created with clustered_lights_shadows, every light shadowed by one of 64 static synthetic cube maps
+(64 x 64 texels a face).  Host lights get the map pointers with set_lights every frame and the clusterer computes the
+shadow transforms; device lights bind the transforms (the reference's, computed once: a point light's depends only on
+its range) and the pointers with the lights, and the clustering pass moves them into cluster order.
 
 Two light lists: 4096 input lights (all in view), and 16384 input lights of which 4096 are kept.  Under torchrun, one
 rank per GPU, row-sharded frames with every rank binding its own copy of the lights; the sharded rate is that of the
@@ -47,6 +52,28 @@ def light_list(n):
                                                                     extra.outer_cone))])
 
 
+SHADOW_RES = 64
+SHADOW_MAPS = 64
+
+
+def shadow_inputs(scene, lights):
+    """(maps tensor, (N,) int64 pointers, (N, 16) float32 transforms in input order) for the --shadows runs.  The
+    transforms are the host clusterer's, put back in input order through distinct stand-in pointers."""
+    n = len(lights.color)
+    rng = np.random.default_rng(7)
+    maps = torch.from_numpy(rng.integers(0, 3000, (SHADOW_MAPS, 6, SHADOW_RES, SHADOW_RES)).astype(np.int16)).cuda()
+    pointers = maps.data_ptr() + 2 * 6 * SHADOW_RES * SHADOW_RES * (np.arange(n, dtype=np.int64) % SHADOW_MAPS)
+    host = viewer.Viewer(W, H, cuda_device=-1, light_shadows=True, shadow_resolution=SHADOW_RES)
+    host.set_camera(scene.projection, scene.view)
+    host.set_lights(lights)
+    host.set_light_shadow_maps(list(range(1, n + 1)))
+    t, m = host.light_shadow_prep()
+    host.close()
+    transforms = np.zeros((n, 16), np.float32)
+    transforms[m.astype(np.int64) - 1] = t
+    return maps, pointers, transforms
+
+
 def timed(v, stream, frames, step):
     """(ms of `frames` frames of step(v, i) after FILL untimed ones, host ms per frame spent in the step calls)."""
     for i in range(FILL):
@@ -70,6 +97,7 @@ def timed(v, stream, frames, step):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=100)
+    ap.add_argument("--shadows", action="store_true", help="shadowed lights with static synthetic maps")
     args = ap.parse_args()
     distributed = "RANK" in os.environ
     if distributed:
@@ -81,14 +109,22 @@ def main():
     scene = synth.make_scene(W, H)
     dev = device_gbuffers(W, H)
     bands = viewer.band_partition(H, world) if world > 1 else None
-    result = {"workload": "c3: 3840x2160, bloom + tonemap, device G-buffer every frame, lights moved on the device every frame",
+    result = {"workload": "c3: 3840x2160, bloom + tonemap, device G-buffer every frame, lights moved on the device every frame" +
+                          (f", every light shadowed ({SHADOW_RES}^2 cube maps, static)" if args.shadows else ""),
               "frames_timed": args.frames, "fill_frames": FILL, "ranks": world, "gpu": card, "runs": []}
+    shadow_cfg = dict(light_shadows=True, shadow_resolution=SHADOW_RES) if args.shadows else {}
 
     for n in (4096, 16384):
         lights = light_list(n)
+        if args.shadows:
+            maps, pointers, transforms = shadow_inputs(scene, lights)
+            shadow_args = dict(shadow_transforms=torch.from_numpy(transforms).cuda(), shadow_maps=torch.from_numpy(pointers).cuda())
         for mode in ("host lights", "device lights"):
             def make(extra):
-                return sharded.make_viewer(W, H, scene, lights, scene.view, bands=bands, **extra)
+                v = sharded.make_viewer(W, H, scene, lights, scene.view, bands=bands, **shadow_cfg, **extra)
+                if args.shadows:
+                    v.set_light_shadow_maps(pointers.tolist())
+                return v
 
             def stepper():
                 state = {"viewer": None}
@@ -100,11 +136,13 @@ def main():
                         state["viewer"] = v
                         state["gbs"] = [v.device_gbuffer(*g) for g in dev]
                         if mode == "device lights":
-                            v.set_lights_device(**d)
+                            v.set_lights_device(**d, **(shadow_args if args.shadows else {}))
                     d["position"].add_(phase)  # the lights' own per-frame update, on the device
                     if mode == "host lights":
                         v.set_lights(synth.Lights(lights.color, d["position"].cpu().numpy(), lights.is_point, lights.rot, lights.inner_cone,
                                                   lights.outer_cone))
+                        if args.shadows:
+                            v.set_light_shadow_maps(pointers.tolist())
                     v.render_frame_device(state["gbs"][i % 2])
                 return step
 
