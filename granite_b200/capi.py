@@ -105,7 +105,8 @@ class GrbLightShadows(C.Structure):
 ENTRY_POINTS = [
     "grb_abi_version", "grb_init", "grb_last_error_string",
     "grb_cluster_spot_transform", "grb_cluster_cull_setup", "grb_cluster_binning", "grb_cluster_binning_rows", "grb_cluster_binning_rows_counted",
-    "grb_cluster_z_range", "grb_light_prep", "grb_light_prep_shadowed", "grb_light_prep_scratch_bytes",
+    "grb_cluster_z_range", "grb_light_prep", "grb_light_prep_shadowed", "grb_light_prep_counted",
+    "grb_light_prep_shadowed_counted", "grb_light_prep_scratch_bytes",
     "grb_cluster_build", "grb_cluster_decal_binning", "grb_fog_light_density", "grb_fog_accumulate", "grb_deferred_lighting", "grb_deferred_lighting_blocks", "grb_deferred_lighting_scheduled", "grb_deferred_lighting_shadowed", "grb_lighting_schedule_bytes", "grb_debug_cluster_indices", "grb_lighting_row_cost",
     "grb_bloom_threshold", "grb_bloom_threshold_downsample", "grb_bloom_threshold_downsample_to_peers", "grb_bloom_downsample", "grb_bloom_downsample_to_peers", "grb_peer_wait", "grb_bloom_upsample", "grb_bloom_upsample_exact",
     "grb_luminance", "grb_luminance_grid", "grb_luminance_finalize", "grb_bloom_tail", "grb_bloom_tail_ex", "grb_tonemap",

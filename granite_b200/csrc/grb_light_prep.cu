@@ -11,6 +11,8 @@
 //   3. pack_kernel, one thread per slot of GRB_MAX_CLUSTER_LIGHTS: the visible count is where the culled keys begin
 //      (a binary search of the sorted keys), and slot s < count packs sorted light s (grb_light_prep_shadowed: with its
 //      shadow transform and map).
+// The _counted forms read the list's live length on the device: step 1 gives every entry past it the culled key without
+// loading it, so steps 2 and 3 are unchanged and never reach those entries.
 #include "grb_common.cuh"
 #include "grb_light_prep.cuh"
 
@@ -25,15 +27,16 @@ namespace
 constexpr int kMaxInputLights = 65536;
 constexpr int kPackThreads = 256;
 
-__global__ void __launch_bounds__(256) cull_key_kernel(GrbLightList lights, GrbLightPrepView view, unsigned long long *__restrict__ keys,
-                                                       uint32_t *__restrict__ values)
+// Counted: only the first lp::live_count(*input_count, lights.count) entries are lights (grb_light_prep[_shadowed]_counted);
+// the <false> form keys every entry.
+template <bool Counted>
+__global__ void __launch_bounds__(256) cull_key_kernel(GrbLightList lights, const int32_t *__restrict__ input_count, GrbLightPrepView view,
+                                                       unsigned long long *__restrict__ keys, uint32_t *__restrict__ values)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= lights.count)
 		return;
-	const lp::Light L = lp::load_light(lights, i);
-	const bool vis = !view.frustum_culling || lp::visible(L, view.planes);
-	keys[i] = ((unsigned long long)(vis ? 0u : 1u) << 32) | lp::radix_key(lp::sort_key(L, view.camera_front));
+	keys[i] = lp::cull_key(lights, view, i, Counted ? lp::live_count(*input_count, lights.count) : lights.count);
 	values[i] = (uint32_t)i;
 }
 
@@ -138,11 +141,11 @@ extern "C" uint64_t grb_light_prep_scratch_bytes(int32_t max_lights)
 
 namespace
 {
-// grb_light_prep and grb_light_prep_shadowed: the checks of grb_light_prep, then the three steps; shadows null = the
-// unshadowed pack kernel
-int32_t light_prep(const char *fn, const GrbLightList *lights, const GrbLightShadowList *shadows, const GrbLightPrepView *view,
-                   GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms,
-                   const void **shadow_maps, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+// grb_light_prep[_shadowed][_counted]: the checks of grb_light_prep, then the three steps; shadows null = the
+// unshadowed pack kernel, input_count null = every entry of the list is a light
+int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowList *shadows,
+                   const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges,
+                   float *shadow_transforms, const void **shadow_maps, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
 {
 	if (!lights || !view || !records || !model || !type_mask || !z_ranges || !device_count || lights->count < 0 || lights->count > kMaxInputLights ||
 	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone ||
@@ -161,6 +164,11 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const GrbLightSha
 		set_last_error((std::string(fn) + ": the output transforms, the map array or the output maps are not 8-byte aligned").c_str());
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
+	if ((uintptr_t)input_count & 3)
+	{
+		set_last_error((std::string(fn) + ": the input count is not 4-byte aligned").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
 	const int n = lights->count;
 	ScratchLayout l;
 	if (!scratch_layout(n, l))
@@ -176,7 +184,10 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const GrbLightSha
 	cudaStream_t s = as_stream(stream);
 	if (n > 0)
 	{
-		cull_key_kernel<<<(n + 255) / 256, 256, 0, s>>>(*lights, *view, keys_in, values_in);
+		if (input_count)
+			cull_key_kernel<true><<<(n + 255) / 256, 256, 0, s>>>(*lights, input_count, *view, keys_in, values_in);
+		else
+			cull_key_kernel<false><<<(n + 255) / 256, 256, 0, s>>>(*lights, nullptr, *view, keys_in, values_in);
 		int32_t r = check_launch((std::string(fn) + ": cull").c_str());
 		if (r != GRB_OK)
 			return r;
@@ -198,7 +209,7 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const GrbLightSha
 extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
                                   uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
 {
-	return light_prep("grb_light_prep", lights, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count, scratch,
+	return light_prep("grb_light_prep", lights, nullptr, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count, scratch,
 	                  scratch_bytes, stream);
 }
 
@@ -211,6 +222,33 @@ extern "C" int32_t grb_light_prep_shadowed(const GrbLightList *lights, const Grb
 		set_last_error("grb_light_prep_shadowed: a null shadow table");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	return light_prep("grb_light_prep_shadowed", lights, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out, shadow_maps_out,
-	                  device_count, scratch, scratch_bytes, stream);
+	return light_prep("grb_light_prep_shadowed", lights, nullptr, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out,
+	                  shadow_maps_out, device_count, scratch, scratch_bytes, stream);
+}
+
+extern "C" int32_t grb_light_prep_counted(const GrbLightList *lights, const int32_t *input_count, const GrbLightPrepView *view, GrbPositionalLight *records,
+                                          float *model, uint32_t *type_mask, uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes,
+                                          void *stream)
+{
+	if (!input_count)
+	{
+		set_last_error("grb_light_prep_counted: a null input count");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return light_prep("grb_light_prep_counted", lights, input_count, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count,
+	                  scratch, scratch_bytes, stream);
+}
+
+extern "C" int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowList *shadows,
+                                                   const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
+                                                   uint32_t *z_ranges, float *shadow_transforms_out, const void **shadow_maps_out, int32_t *device_count,
+                                                   void *scratch, uint64_t scratch_bytes, void *stream)
+{
+	if (!input_count || !shadows)
+	{
+		set_last_error("grb_light_prep_shadowed_counted: a null input count or shadow table");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return light_prep("grb_light_prep_shadowed_counted", lights, input_count, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out,
+	                  shadow_maps_out, device_count, scratch, scratch_bytes, stream);
 }

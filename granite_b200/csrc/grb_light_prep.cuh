@@ -173,6 +173,22 @@ __host__ __device__ inline uint32_t radix_key(float key)
 	return (u >> 31) ? ~u : (u | 0x80000000u);
 }
 
+// The live length of a list of `capacity` entries whose count the caller wrote in device memory: a value written on the
+// device cannot be refused, so one outside 0..capacity is clamped.
+__host__ __device__ inline int live_count(int32_t count, int capacity) { return count < 0 ? 0 : (count > capacity ? capacity : count); }
+
+// The cull kernel's 33-bit sort key of input light i when the first `live` entries are the light list: bit 32 set for a
+// light the frustum culls, bits 0..31 the radix code of its sort key.  An entry at or past `live` is never loaded (it
+// may hold anything) and gets the bare culled key, so it sorts behind every visible light and no slot packs it.
+__host__ __device__ inline unsigned long long cull_key(const GrbLightList &lights, const GrbLightPrepView &view, int i, int live)
+{
+	if (i >= live)
+		return 1ull << 32;
+	const Light L = load_light(lights, i);
+	const bool vis = !view.frustum_culling || visible(L, view.planes);
+	return ((unsigned long long)(vis ? 0u : 1u) << 32) | radix_key(sort_key(L, view.camera_front));
+}
+
 // PointLight / SpotLight::get_shader_info, the model row (set_point_model_transform / SpotLight::build_model_matrix) and
 // the Z-slice range (point_light_z_range / spot_light_z_range, then compute_uint_range)
 __host__ __device__ inline void pack(const Light &L, const GrbLightPrepView &view, GrbPositionalLight &rec, float model[12], uint32_t zr[2])

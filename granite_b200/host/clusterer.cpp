@@ -446,20 +446,32 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 		if (src.ready)
 			Vulkan::cuda_ok(cudaStreamWaitEvent(stream, static_cast<cudaEvent_t>(src.ready), 0), "cudaStreamWaitEvent(lights ready)");
 		const GrbClusterBuffers buf = get_cluster_buffers();
+		auto *records = const_cast<GrbPositionalLight *>(buf.lights);
+		auto *model = const_cast<float *>(buf.model);
+		auto *type_mask = const_cast<uint32_t *>(buf.type_mask);
+		auto *z_ranges = const_cast<uint32_t *>(buf.z_ranges);
+		void *s = cmd.get_stream_handle();
 		if (enable_shadows)
 		{
 			// the shadow tables where the lighting pass reads them: packed_size(slots) and packed_offset_shadow_maps(slots)
 			const GrbLightShadows out = get_light_shadows();
-			cmd.check(grb_light_prep_shadowed(&src.list, &src.shadows, &device_view, const_cast<GrbPositionalLight *>(buf.lights),
-			                                  const_cast<float *>(buf.model), const_cast<uint32_t *>(buf.type_mask), const_cast<uint32_t *>(buf.z_ranges),
-			                                  const_cast<float *>(out.transforms), const_cast<const void **>(out.maps), src.count, src.scratch,
-			                                  src.scratch_bytes, cmd.get_stream_handle()),
-			          "grb_light_prep_shadowed");
+			auto *transforms = const_cast<float *>(out.transforms);
+			auto *maps = const_cast<const void **>(out.maps);
+			if (src.input_count)
+				cmd.check(grb_light_prep_shadowed_counted(&src.list, src.input_count, &src.shadows, &device_view, records, model, type_mask, z_ranges,
+				                                          transforms, maps, src.count, src.scratch, src.scratch_bytes, s),
+				          "grb_light_prep_shadowed_counted");
+			else
+				cmd.check(grb_light_prep_shadowed(&src.list, &src.shadows, &device_view, records, model, type_mask, z_ranges, transforms, maps, src.count,
+				                                  src.scratch, src.scratch_bytes, s),
+				          "grb_light_prep_shadowed");
 		}
+		else if (src.input_count)
+			cmd.check(grb_light_prep_counted(&src.list, src.input_count, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch,
+			                                 src.scratch_bytes, s),
+			          "grb_light_prep_counted");
 		else
-			cmd.check(grb_light_prep(&src.list, &device_view, const_cast<GrbPositionalLight *>(buf.lights), const_cast<float *>(buf.model),
-			                         const_cast<uint32_t *>(buf.type_mask), const_cast<uint32_t *>(buf.z_ranges), src.count, src.scratch, src.scratch_bytes,
-			                         cmd.get_stream_handle()),
+			cmd.check(grb_light_prep(&src.list, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch, src.scratch_bytes, s),
 			          "grb_light_prep");
 		if (src.consumed)
 			Vulkan::cuda_ok(cudaEventRecord(static_cast<cudaEvent_t>(src.consumed), stream), "cudaEventRecord(lights consumed)");

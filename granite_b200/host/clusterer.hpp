@@ -96,10 +96,14 @@ public:
 	// arrays and `consumed` recorded after the last.  With shadows enabled the caller also gives each input light's
 	// shadow transform and map (`shadows`, read under the same events): the prep (grb_light_prep_shadowed) moves them into
 	// cluster order, into the tables get_light_shadows() points at.  The transforms are the caller's, never computed here.
+	// `input_count` (device, or null = all list.count entries are lights) makes list.count a capacity: the prep
+	// (grb_light_prep[_shadowed]_counted) reads the live length under the same events; refresh() still sizes the frame
+	// from the capacity.
 	struct DeviceLightSource
 	{
 		GrbLightList list = {};
 		GrbLightShadowList shadows = {};
+		const int32_t *input_count = nullptr;
 		void *ready = nullptr, *consumed = nullptr;
 		void *scratch = nullptr; // grb_light_prep_scratch_bytes(list.count) or more
 		size_t scratch_bytes = 0;

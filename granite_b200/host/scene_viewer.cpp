@@ -1072,6 +1072,7 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 	v->cluster.set_device_lights(nullptr);
 	v->device_prep_rendered = false;
 	v->device_lights.shadows = {};
+	v->device_lights.input_count = nullptr;
 	v->shadow_map_events.ready = v->shadow_map_events.consumed = nullptr;
 	v->light_storage.clear();
 	v->scene_lights.clear();
@@ -1176,6 +1177,7 @@ int32_t bind_device_lights(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhD
 	d.list.cutoff_range = l->cutoff_range;
 	d.shadows.transforms = sh ? sh->transforms : nullptr;
 	d.shadows.maps = sh ? reinterpret_cast<const void *const *>(sh->maps) : nullptr;
+	d.input_count = nullptr; // a new list: every entry is live until grbh_viewer_set_light_count_device
 	d.ready = l->ready;
 	d.consumed = l->consumed;
 	d.count = static_cast<int32_t *>(v->light_scratch);
@@ -1221,6 +1223,29 @@ extern "C" int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *v, const G
 		return fail(fn + "host-only viewer (no CUDA device)");
 	GRBH_TRY
 	return bind_device_lights(v, l, shadows, fn);
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_light_count_device(GrbhViewer *v, const int32_t *count)
+{
+	const std::string fn = "grbh_viewer_set_light_count_device: ";
+	if (!v)
+		return fail(fn + "null viewer");
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	if (!v->cluster.has_device_lights())
+		return fail(fn + "no device light list is bound (grbh_viewer_set_lights_device[_shadowed] first)");
+	if ((uintptr_t)count & 3)
+		return fail(fn + "the count is not 4-byte aligned");
+	GRBH_TRY
+	if (count)
+	{
+		cudaSetDevice(v->device->get_device_index());
+		if (!is_viewer_device_memory(v, fn, "count", count, sizeof(int32_t)))
+			return -1;
+	}
+	v->device_lights.input_count = count;
+	return 0;
 	GRBH_CATCH
 }
 

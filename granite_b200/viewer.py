@@ -76,6 +76,7 @@ def lib() -> C.CDLL:
         _lib.grbh_viewer_set_exposure.argtypes = [C.c_void_p, C.c_float]
         _lib.grbh_viewer_set_output_images.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         _lib.grbh_viewer_acquire_output.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        _lib.grbh_viewer_set_light_count_device.argtypes = [C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -413,7 +414,7 @@ class Viewer:
         _check(lib().grbh_viewer_set_lights(self._h, C.byref(l)), "grbh_viewer_set_lights")
 
     def set_lights_device(self, color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, ready=None, consumed=None,
-                          shadow_transforms=None, shadow_maps=None, maps_ready=None, maps_consumed=None):
+                          shadow_transforms=None, shadow_maps=None, maps_ready=None, maps_consumed=None, count=None):
         """Binds a light list in device memory (grbh_viewer_set_lights_device) from the next frame until the next
         set_lights[_device] call: torch CUDA tensors on the viewer's device, contiguous, in synth.Lights' shapes --
         color and position (N, 3) float32, is_point (N,) bool or uint8, rotation (N, 3, 3) float32 column-major,
@@ -426,7 +427,12 @@ class Viewer:
         the same order: shadow_transforms (N, 16) or (N, 4, 4) float32, column-major, the matrix the light's map was
         rendered with; shadow_maps (N,) int64 of map data_ptr()s, 0 = no shadow.  Both are read with the lights, under
         ready / consumed.  maps_ready: a torch.cuda.Event the lighting pass waits on before it samples the maps;
-        maps_consumed: one the viewer records behind the lighting pass's last read of them."""
+        maps_consumed: one the viewer records behind the lighting pass's last read of them.
+
+        count: a torch CUDA int32 tensor of one element, on the viewer's device, holding the list's live length
+        (grbh_viewer_set_light_count_device).  N is then a capacity: each frame reads the count under ready / consumed
+        and renders the first min(max(count, 0), N) lights, so a GPU pass that spawns, kills or compacts lights can
+        rewrite it between frames without a host sync.  Entries past it are never read.  Without it all N are lights."""
         import torch
 
         shadowed = shadow_transforms is not None or shadow_maps is not None
@@ -445,6 +451,13 @@ class Viewer:
                                  f"{' or '.join(str(d) for d in dtypes)}, got {tuple(t.shape)} {t.dtype}")
             if not t.is_contiguous():
                 raise ValueError(f"set_lights_device: {name} must be contiguous")
+        if count is not None:
+            if not isinstance(count, torch.Tensor) or not count.is_cuda:
+                raise ValueError("set_lights_device: count must be a torch CUDA tensor")
+            if count.numel() != 1 or count.dtype != torch.int32:
+                raise ValueError(f"set_lights_device: count must be one torch.int32 element, got {tuple(count.shape)} {count.dtype}")
+            if count.device != color.device:
+                raise ValueError(f"set_lights_device: count is on {count.device}, the lights on {color.device}")
         if not shadowed and (maps_ready is not None or maps_consumed is not None):
             raise ValueError("set_lights_device: maps_ready / maps_consumed need shadow_transforms and shadow_maps")
         for ev in (ready, consumed, maps_ready, maps_consumed):
@@ -463,6 +476,9 @@ class Viewer:
         else:
             _check(lib().grbh_viewer_set_lights_device(self._h, C.byref(l)), "grbh_viewer_set_lights_device")
             self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone)
+        if count is not None:
+            _check(lib().grbh_viewer_set_light_count_device(self._h, count.data_ptr()), "grbh_viewer_set_light_count_device")
+            self._device_lights += (count,)
 
     def init_collectives(self, unique_id: bytes, rank: int, world: int):
         buf = (C.c_uint8 * 128).from_buffer_copy(unique_id)

@@ -220,6 +220,21 @@ typedef struct GrbLightShadowList
 int32_t grb_light_prep_shadowed(const GrbLightList *lights, const GrbLightShadowList *shadows, const GrbLightPrepView *view,
                                 GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms_out,
                                 const void **shadow_maps_out, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream);
+/* grb_light_prep[_shadowed] for a list whose length is known only on the device: lights->count is its capacity, and
+ * the first live = min(max(*input_count, 0), lights->count) entries are the lights (a count written on the device cannot
+ * be refused, so it is clamped).  input_count: device, 4-byte aligned, read by the cull kernel on `stream`.  Entries
+ * [live, capacity) are never read, not even their shadow transforms or maps.  The capacity sizes everything the host
+ * sizes: the radix sort, the scratch (grb_light_prep_scratch_bytes(capacity)) and slots = min(capacity,
+ * GRB_MAX_CLUSTER_LIGHTS); the outputs are the bytes grb_light_prep[_shadowed] gives for a list of the first `live`
+ * lights in slots [0, count) and the empty slot in [count, slots).  Same three launches.
+ * GRB_ERR_INVALID_ARGUMENT: what grb_light_prep[_shadowed] refuses, a null or misaligned input_count. */
+int32_t grb_light_prep_counted(const GrbLightList *lights, const int32_t *input_count, const GrbLightPrepView *view, GrbPositionalLight *records,
+                               float *model, uint32_t *type_mask, uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes,
+                               void *stream);
+int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowList *shadows,
+                                        const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges,
+                                        float *shadow_transforms_out, const void **shadow_maps_out, int32_t *device_count, void *scratch,
+                                        uint64_t scratch_bytes, void *stream);
 
 /* Volumetric-decal binning over the clusterer's tile grid: LightClusterer::update_bindless_mask_buffer_decal_gpu
  * (clusterer.cpp:1391-1461) + clusterer_bindless_binning_decal.comp.  mvps: num_decals x mat4 (column-major, device) =

@@ -165,6 +165,15 @@ int32_t grbh_viewer_set_lights_device(GrbhViewer *viewer, const GrbhDeviceLights
  * a viewer created without clustered_lights_shadows, null tables with count > 0, a host-only viewer, arrays or tables
  * that are not device memory of the viewer's device. */
 int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *viewer, const GrbhDeviceLights *lights, const GrbhDeviceLightShadows *shadows);
+/* Gives the device light list bound now (shadowed or not) a length that lives on the device: its `count` becomes the
+ * capacity, and every frame's clustering pass reads *count under the lights' ready / consumed events, so a GPU pass may
+ * rewrite it between frames with no host read.  Entries [0, live) are the lights, live = min(max(*count, 0), capacity)
+ * (a value written on the device cannot be refused, so it is clamped); entries [live, capacity) are never read.  The
+ * frame equals the frame of the first `live` lights bound without a count.  count: device memory of the viewer's device,
+ * 4-byte aligned, alive while frames that read it are in flight; NULL goes back to every bound entry being live.
+ * grbh_viewer_set_lights[_device[_shadowed]] clear it: a new binding is a new list.  Refused: a null viewer, a host-only
+ * viewer, no device light list bound, a count that is not 4-byte aligned or not device memory of the viewer's device. */
+int32_t grbh_viewer_set_light_count_device(GrbhViewer *viewer, const int32_t *count);
 int32_t grbh_viewer_set_exposure(GrbhViewer *viewer, float exposure);
 /* Shadow maps of the lights of the last grbh_viewer_set_lights call, in THAT order: `count` device pointers (host array),
  * each D16_UNORM of resolution^2 texels (spot) or 6 x resolution^2 (point, faces +X -X +Y -Y +Z -Z); null = no shadow.

@@ -6,13 +6,24 @@ moved every frame by a small torch op on the device, by where the light prep run
 - "device lights": set_lights_device binds the tensors once; every frame's clustering pass culls, sorts and packs them
   on the GPU.
 
-    python tools/device_lights_times.py [--frames 100] [--shadows]
-    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows]
+    python tools/device_lights_times.py [--frames 100] [--shadows | --live-count]
+    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows | --live-count]
 
 --shadows: viewers created with clustered_lights_shadows, every light shadowed by one of 64 static synthetic cube maps
 (64 x 64 texels a face).  Host lights get the map pointers with set_lights every frame and the clusterer computes the
 shadow transforms; device lights bind the transforms (the reference's, computed once: a point light's depends only on
 its range) and the pointers with the lights, and the clustering pass moves them into cluster order.
+
+--live-count: a particle-style list whose length is known only on the device.  16384 particle lights, each alive for a
+lifetime of its own in a cycle of its own, so that about half are alive and the set changes every frame.  Every frame a
+torch op compacts the alive particles into a light list and writes its length, with a cumsum scatter and no host sync.
+Three ways to hand that list over are timed in the same run:
+- "device count": the list and its count are bound once (set_lights_device(..., count=)); the clustering pass reads
+  the count on the device;
+- "count read back": the count is read to the host and the list rebound with that length every frame;
+- "parked": no compaction: the whole capacity is bound and dead particles are parked behind the camera, where the
+  frustum cull drops them.
+The torch ops run on the caller's stream and the viewer waits on them through the lights' ready / consumed events.
 
 Two light lists: 4096 input lights (all in view), and 16384 input lights of which 4096 are kept.  Under torchrun, one
 rank per GPU, row-sharded frames with every rank binding its own copy of the lights; the sharded rate is that of the
@@ -74,6 +85,94 @@ def shadow_inputs(scene, lights):
     return maps, pointers, transforms
 
 
+PARTICLES = 16384
+
+
+def particles():
+    """(lights, per-particle cycle, per-particle lifetime): 16384 particle lights in view, alive at frame f when
+    (f + offset) % cycle < lifetime, which holds for about half of them in every frame."""
+    lights = synth.make_lights(PARTICLES, spot_fraction=0.0, aspect=W / H)
+    rng = np.random.default_rng(11)
+    cycle = rng.integers(8, 64, PARTICLES)
+    lifetime = np.maximum(1, (cycle * rng.uniform(0.3, 0.7, PARTICLES)).astype(np.int64))
+    offset = rng.integers(0, 64, PARTICLES)
+    return lights, cycle, lifetime, offset
+
+
+def live_count_stepper(mode, lights, cycle, lifetime, offset):
+    """step(v, i) for one --live-count mode: the particle update, the compaction (or the parking) and the frame."""
+    n = PARTICLES
+    src = cases.to_device(lights)
+    cycle_t, lifetime_t, offset_t = (torch.from_numpy(a).cuda() for a in (cycle, lifetime, offset))
+    # the compacted list, one row more than the capacity: dead particles are scattered into the last row
+    out = {k: torch.empty((n + 1, *t.shape[1:]), dtype=t.dtype, device="cuda") for k, t in src.items()}
+    bound = {k: t[:n] for k, t in out.items()}
+    parked = {k: t.clone() for k, t in src.items()}
+    count = torch.zeros(1, dtype=torch.int32, device="cuda")
+    ready, consumed = torch.cuda.Event(), torch.cuda.Event()
+    state = {"viewer": None}
+
+    def step(v, i):
+        if state["viewer"] is not v:
+            state["viewer"] = v
+            state["gbs"] = [v.device_gbuffer(*g) for g in state["dev"]]
+            if mode == "device count":
+                v.set_lights_device(**bound, ready=ready, consumed=consumed, count=count)
+            elif mode == "parked":
+                v.set_lights_device(**parked, ready=ready, consumed=consumed)
+        else:
+            torch.cuda.current_stream().wait_event(consumed)
+        alive = (i + offset_t) % cycle_t < lifetime_t
+        if mode == "parked":
+            for k in parked:
+                parked[k].copy_(src[k])
+            parked["position"][:, 2].masked_fill_(~alive, 1000.0)  # behind the eye: culled
+        else:
+            csum = torch.cumsum(alive, 0, dtype=torch.int32)
+            dest = torch.where(alive, csum.long() - 1, n)
+            for k in out:
+                out[k].index_copy_(0, dest, src[k])
+            count.copy_(csum[-1:])
+        ready.record()
+        if mode == "count read back":
+            k = int(count.item())
+            v.set_lights_device(**{name: t[:k] for name, t in out.items()}, ready=ready, consumed=consumed)
+        v.render_frame_device(state["gbs"][i % 2])
+
+    return step, state
+
+
+def live_count_runs(args, scene, dev, bands, card, distributed, rank, world):
+    lights, cycle, lifetime, offset = particles()
+    closer = sharded.close_sharded if distributed else (lambda v: v.close())
+    runs = []
+    for mode in ("device count", "count read back", "parked"):
+        times = []
+        for timestamps in (False, True):
+            step, state = live_count_stepper(mode, lights, cycle, lifetime, offset)
+            state["dev"] = dev
+            stream = torch.cuda.Stream()
+            v = sharded.make_viewer(W, H, scene, synth.make_lights(0), scene.view, bands=bands, stream=stream.cuda_stream, timestamps=timestamps)
+            times.append(timed(v, stream, args.frames, step))
+            if timestamps:
+                t, c = v.collect_timings().get("clustering-bindless", (0.0, 0))
+            else:
+                kept = v.light_prep()[0]
+            closer(v)
+        ms, host_ms = times[0]
+        run = {"capacity": PARTICLES, "kept_lights_last_frame": kept, "mode": mode, "ms": ms, "host_ms_per_frame": round(host_ms, 4),
+               "clustering_pass_ms": round(t / max(c, 1), 4), "gpu": card}
+        if distributed:
+            gathered = [None] * world
+            torch.distributed.all_gather_object(gathered, dict(run, rank=rank))
+            run = {"capacity": PARTICLES, "mode": mode, "frames_per_s": round(args.frames / (max(g["ms"] for g in gathered) * 1e-3), 2),
+                   "ranks": gathered}
+        else:
+            run["frames_per_s"] = round(args.frames / (ms * 1e-3), 2)
+        runs.append(run)
+    return runs
+
+
 def timed(v, stream, frames, step):
     """(ms of `frames` frames of step(v, i) after FILL untimed ones, host ms per frame spent in the step calls)."""
     for i in range(FILL):
@@ -98,7 +197,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=100)
     ap.add_argument("--shadows", action="store_true", help="shadowed lights with static synthetic maps")
+    ap.add_argument("--live-count", action="store_true", help="a compacted particle list whose length is known only on the device")
     args = ap.parse_args()
+    if args.shadows and args.live_count:
+        ap.error("--shadows and --live-count are separate workloads")
     distributed = "RANK" in os.environ
     if distributed:
         rank, world, local = sharded.init_ranks(allow_shared=False)
@@ -112,6 +214,15 @@ def main():
     result = {"workload": "c3: 3840x2160, bloom + tonemap, device G-buffer every frame, lights moved on the device every frame" +
                           (f", every light shadowed ({SHADOW_RES}^2 cube maps, static)" if args.shadows else ""),
               "frames_timed": args.frames, "fill_frames": FILL, "ranks": world, "gpu": card, "runs": []}
+    if args.live_count:
+        result["workload"] = (f"c3: 3840x2160, bloom + tonemap, device G-buffer every frame, {PARTICLES} particle lights of which about half "
+                              "are alive, compacted on the device every frame")
+        result["runs"] = live_count_runs(args, scene, dev, bands, card, distributed, rank, world)
+        if rank == 0:
+            print(json.dumps(result), flush=True)
+        if distributed:
+            torch.distributed.destroy_process_group()
+        return
     shadow_cfg = dict(light_shadows=True, shadow_resolution=SHADOW_RES) if args.shadows else {}
 
     for n in (4096, 16384):
