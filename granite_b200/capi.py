@@ -98,6 +98,15 @@ class GrbFogParameters(C.Structure):
                 ("slice_z_log2_scale", C.c_float), ("density_mod", C.c_float), ("in_scatter_strength", C.c_float)]
 
 
+class GrbLightList(C.Structure):
+    """A light list as grb_light_prep / grb_light_list_to_peers take it: device arrays in synth.Lights' layout."""
+    _fields_ = [("count", C.c_int32), ("color", C.c_void_p), ("position", C.c_void_p), ("is_point", C.c_void_p), ("rotation", C.c_void_p),
+                ("inner_cone", C.c_void_p), ("outer_cone", C.c_void_p), ("cutoff_range", C.c_float)]
+
+
+MAX_LIGHT_LIST = 65536  # GRB_MAX_LIGHT_LIST
+
+
 class GrbLightShadows(C.Structure):
     _fields_ = [("transforms", C.c_void_p), ("maps", C.c_void_p), ("resolution", C.c_int32), ("pcf_wide", C.c_int32)]
 
@@ -112,7 +121,7 @@ ENTRY_POINTS = [
     "grb_luminance", "grb_luminance_grid", "grb_luminance_finalize", "grb_bloom_tail", "grb_bloom_tail_ex", "grb_tonemap",
     "grb_pq10_encode", "grb_smaa_edge_detection", "grb_smaa_edge_detection_to_peers", "grb_smaa_blend_weights", "grb_smaa_neighborhood_blend", "grb_fsr_easu_constants", "grb_fsr_upscale", "grb_fsr_sharpen", "grb_fxaa", "grb_taa_resolve", "grb_taa_resolve_to_peers",
     "grb_present_rows_to_peer", "grb_deferred_lighting_stripes", "grb_hdr_rows_to_peers",
-    "grb_gbuffer_copy_rows", "grb_gbuffer_slot_layout", "grb_gbuffer_rows_to_peers",
+    "grb_gbuffer_copy_rows", "grb_gbuffer_slot_layout", "grb_gbuffer_rows_to_peers", "grb_light_slot_layout", "grb_light_list_to_peers",
 ]
 
 _lib = None
@@ -175,6 +184,8 @@ def lib() -> C.CDLL:
             "grb_gbuffer_copy_rows": [C.POINTER(GrbGBufferPlanes), C.POINTER(GrbGBufferPlanes), C.POINTER(GrbRows), I, P],
             "grb_gbuffer_slot_layout": [C.POINTER(GrbGBufferPlanes), P, C.POINTER(GrbGBufferPlanes), C.POINTER(C.c_uint64)],
             "grb_gbuffer_rows_to_peers": [C.POINTER(GrbGBufferPlanes), P, P, C.POINTER(GrbRows), C.POINTER(C.c_int32), I, I, C.c_uint32, P, P],
+            "grb_light_slot_layout": [P, C.POINTER(GrbLightList), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)],
+            "grb_light_list_to_peers": [C.POINTER(GrbLightList), P, P, P, I, I, C.c_uint32, P, P],
         }
         for name, args in sig.items():
             fn = getattr(_lib, name)

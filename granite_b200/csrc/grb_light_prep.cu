@@ -13,8 +13,12 @@
 //      shadow transform and map).
 // The _counted forms read the list's live length on the device: step 1 gives every entry past it the culled key without
 // loading it, so steps 2 and 3 are unchanged and never reach those entries.
+//
+// grb_light_list_to_peers pushes a list's live entries from one rank into every rank's light slot (the protocol is
+// grb_peer.cuh's); each receiver then runs the counted prep on its slot, so every rank preps the same bytes.
 #include "grb_common.cuh"
 #include "grb_light_prep.cuh"
+#include "grb_peer.cuh"
 
 #include <cub/device/device_radix_sort.cuh>
 
@@ -24,7 +28,7 @@ namespace grb
 {
 namespace
 {
-constexpr int kMaxInputLights = 65536;
+constexpr int kMaxInputLights = GRB_MAX_LIGHT_LIST;
 constexpr int kPackThreads = 256;
 
 // Counted: only the first lp::live_count(*input_count, lights.count) entries are lights (grb_light_prep[_shadowed]_counted);
@@ -99,6 +103,24 @@ __global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights,
 		type_mask[s >> 5] = word;
 	if (s == 0)
 		*count_out = count;
+}
+
+// One thread per 16-byte chunk of the capacity's six arrays (lp::push_light_chunk), then the count word and the
+// publish.  No slots: a flags-only publish.
+__global__ void __launch_bounds__(256) light_push_kernel(lp::LightPush push, const int32_t *__restrict__ input_count, int capacity, PeerTargets targets)
+{
+	if (targets.data[0])
+	{
+		const int live = input_count ? lp::live_count(*input_count, capacity) : capacity;
+		const int t = blockIdx.x * blockDim.x + threadIdx.x;
+		lp::push_light_chunk(push, live, t, targets.data, targets.count);
+		if (t == 0)
+#pragma unroll
+			for (int r = 0; r < GRB_MAX_PEERS; r++)
+				if (r < targets.count)
+					*reinterpret_cast<int32_t *>(static_cast<uint8_t *>(targets.data[r]) + lp::light_slot_layout().count) = live;
+	}
+	peer_publish(targets);
 }
 
 struct ScratchLayout
@@ -251,4 +273,71 @@ extern "C" int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, c
 	}
 	return light_prep("grb_light_prep_shadowed_counted", lights, input_count, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out,
 	                  shadow_maps_out, device_count, scratch, scratch_bytes, stream);
+}
+
+extern "C" int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t **count_out, uint64_t *bytes)
+{
+	if (!bytes)
+	{
+		set_last_error("grb_light_slot_layout: a null size pointer");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if ((uintptr_t)slot & 15)
+	{
+		set_last_error("grb_light_slot_layout: the slot is not 16-byte aligned");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	const lp::LightSlotLayout l = lp::light_slot_layout();
+	*bytes = l.bytes;
+	auto *base = static_cast<uint8_t *>(slot);
+	auto at = [&](int a) { return base ? base + l.array[a] : nullptr; };
+	if (out)
+	{
+		*out = GrbLightList{};
+		out->count = GRB_MAX_LIGHT_LIST;
+		out->color = reinterpret_cast<const float *>(at(0));
+		out->position = reinterpret_cast<const float *>(at(1));
+		out->is_point = at(2);
+		out->rotation = reinterpret_cast<const float *>(at(3));
+		out->inner_cone = reinterpret_cast<const float *>(at(4));
+		out->outer_cone = reinterpret_cast<const float *>(at(5));
+	}
+	if (count_out)
+		*count_out = base ? reinterpret_cast<int32_t *>(base + l.count) : nullptr;
+	return GRB_OK;
+}
+
+extern "C" int32_t grb_light_list_to_peers(const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
+                                           int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream)
+{
+	const char *fn = "grb_light_list_to_peers";
+	PeerTargets targets;
+	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets, /*flags_only=*/peer_slots == nullptr))
+		return GRB_ERR_INVALID_ARGUMENT;
+	if (!peer_slots)
+	{
+		light_push_kernel<<<1, 256, 0, as_stream(stream)>>>(lp::LightPush{}, nullptr, 0, targets);
+		return check_launch(fn);
+	}
+	if (!lights || lights->count < 0 || lights->count > GRB_MAX_LIGHT_LIST ||
+	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone || !lights->outer_cone)))
+	{
+		set_last_error("grb_light_list_to_peers: a null light list or array, or a count outside 0..GRB_MAX_LIGHT_LIST");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if ((uintptr_t)input_count & 3)
+	{
+		set_last_error("grb_light_list_to_peers: the input count is not 4-byte aligned");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	for (int r = 0; r < peer_count; r++)
+		if ((uintptr_t)peer_slots[r] & 15)
+		{
+			set_last_error("grb_light_list_to_peers: a slot is not 16-byte aligned");
+			return GRB_ERR_INVALID_ARGUMENT;
+		}
+	const lp::LightPush push = lp::light_push(*lights);
+	const unsigned blocks = (unsigned)((push.start[lp::kLightArrays] + 255) / 256);
+	light_push_kernel<<<blocks > 0 ? blocks : 1, 256, 0, as_stream(stream)>>>(push, input_count, lights->count, targets);
+	return check_launch(fn);
 }

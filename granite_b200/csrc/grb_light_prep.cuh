@@ -189,6 +189,121 @@ __host__ __device__ inline unsigned long long cull_key(const GrbLightList &light
 	return ((unsigned long long)(vis ? 0u : 1u) << 32) | radix_key(sort_key(L, view.camera_front));
 }
 
+// The light slot of a row-sharded frame's light channel (grb_light_slot_layout): the count word, then the six arrays of
+// a GrbLightList of GRB_MAX_LIGHT_LIST entries in GrbLightList order, each from a multiple of 256 bytes.
+constexpr int kLightArrays = 6;
+// the element size of array a: color, position, is_point, rotation, inner_cone, outer_cone
+__host__ __device__ inline int light_element_bytes(int a) { return a < 2 ? 12 : (a == 2 ? 1 : (a == 3 ? 36 : 4)); }
+struct LightSlotLayout
+{
+	uint64_t count;
+	uint64_t array[kLightArrays];
+	uint64_t bytes;
+};
+// the offset of array a (a == kLightArrays: the slot's size)
+__host__ __device__ inline uint64_t light_array_offset(int a)
+{
+	uint64_t at = 256;
+	for (int k = 0; k < a; k++)
+		at += ((uint64_t)GRB_MAX_LIGHT_LIST * (uint64_t)light_element_bytes(k) + 255) / 256 * 256;
+	return at;
+}
+__host__ __device__ inline LightSlotLayout light_slot_layout()
+{
+	LightSlotLayout l;
+	l.count = 0;
+	for (int a = 0; a < kLightArrays; a++)
+		l.array[a] = light_array_offset(a);
+	l.bytes = light_array_offset(kLightArrays);
+	return l;
+}
+
+// What the push kernel of grb_light_list_to_peers copies: the six source arrays, laid end to end in 16-byte chunks of
+// which array a owns [start[a], start[a + 1]) (start[kLightArrays] = every chunk of the capacity), and whether array
+// a moves in 16-byte words (vec16) or 4-byte words (vec4) -- both sides aligned -- or else byte by byte.
+struct LightPush
+{
+	const uint8_t *src[kLightArrays];
+	int start[kLightArrays + 1];
+	unsigned vec16, vec4;
+};
+
+// The push of `lights` (count = its capacity): each array's source and chunk range, and the word size both sides allow
+// (the slots are 16-byte aligned and every array of a slot starts on a multiple of 256 bytes).
+inline LightPush light_push(const GrbLightList &lights)
+{
+	LightPush push = {};
+	const void *src[kLightArrays] = { lights.color, lights.position, lights.is_point, lights.rotation, lights.inner_cone, lights.outer_cone };
+	push.start[0] = 0;
+	for (int a = 0; a < kLightArrays; a++)
+	{
+		push.src[a] = static_cast<const uint8_t *>(src[a]);
+		const uintptr_t p = reinterpret_cast<uintptr_t>(src[a]);
+		if ((p & 15) == 0)
+			push.vec16 |= 1u << a;
+		if (light_element_bytes(a) % 4 == 0 && (p & 3) == 0)
+			push.vec4 |= 1u << a;
+		push.start[a + 1] = push.start[a] + (lights.count * light_element_bytes(a) + 15) / 16;
+	}
+	return push;
+}
+
+// Thread t of the push: chunk t's bytes that lie below live x element size of its array, loaded once and stored at the
+// same offset of that array in each of the `count` (<= GRB_MAX_PEERS) slots; nothing at or past it is read.  The loops
+// over the arrays and the slots unroll, so that the kernel indexes its parameters with constants only.
+__host__ __device__ inline void push_light_chunk(const LightPush &p, int live, int t, void *const *slots, int count)
+{
+	if (t >= p.start[kLightArrays])
+		return;
+	int a = 0;
+	const uint8_t *src = p.src[0];
+	int first = 0;
+#pragma unroll
+	for (int k = 1; k < kLightArrays; k++)
+		if (t >= p.start[k])
+		{
+			a = k;
+			src = p.src[k];
+			first = p.start[k];
+		}
+	const uint64_t at = 16ull * (uint64_t)(t - first);
+	const uint64_t end = (uint64_t)live * (uint64_t)light_element_bytes(a);
+	if (at >= end)
+		return;
+	const int n = end - at < 16 ? (int)(end - at) : 16;
+	const uint64_t dst = light_array_offset(a) + at;
+	const uint8_t *s = src + at;
+	if (n == 16 && ((p.vec16 >> a) & 1u))
+	{
+		const uint4 v = *reinterpret_cast<const uint4 *>(s);
+#pragma unroll
+		for (int r = 0; r < GRB_MAX_PEERS; r++)
+			if (r < count)
+				*reinterpret_cast<uint4 *>(static_cast<uint8_t *>(slots[r]) + dst) = v;
+	}
+	else if ((p.vec4 >> a) & 1u)
+	{
+		// n is a multiple of 4 here: the arrays that move in 4-byte words have 4-byte elements
+		for (int j = 0; j < n; j += 4)
+		{
+			const uint32_t v = *reinterpret_cast<const uint32_t *>(s + j);
+#pragma unroll
+			for (int r = 0; r < GRB_MAX_PEERS; r++)
+				if (r < count)
+					*reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(slots[r]) + dst + j) = v;
+		}
+	}
+	else
+		for (int j = 0; j < n; j++)
+		{
+			const uint8_t v = s[j];
+#pragma unroll
+			for (int r = 0; r < GRB_MAX_PEERS; r++)
+				if (r < count)
+					static_cast<uint8_t *>(slots[r])[dst + j] = v;
+		}
+}
+
 // PointLight / SpotLight::get_shader_info, the model row (set_point_model_transform / SpotLight::build_model_matrix) and
 // the Z-slice range (point_light_z_range / spot_light_z_range, then compute_uint_range)
 __host__ __device__ inline void pack(const Light &L, const GrbLightPrepView &view, GrbPositionalLight &rec, float model[12], uint32_t zr[2])

@@ -408,6 +408,34 @@ def gbuffer_rows_to_peers(src, slots, flag_arrays, rows_per_rank, flag_index, ep
                "grb_gbuffer_rows_to_peers")
 
 
+def light_list(color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, count=None) -> capi.GrbLightList:
+    """A GrbLightList over CUDA tensors in synth.Lights' shapes (Viewer.set_lights_device's); count (default: the
+    tensors' length) is the list's capacity."""
+    n = int(color.shape[0]) if count is None else int(count)
+    return capi.GrbLightList(n, *[t.data_ptr() for t in (color, position, is_point, rotation, inner_cone, outer_cone)], float(cutoff))
+
+
+def light_slot_layout(base=None):
+    """grb_light_slot_layout: (the GrbLightList of a slot at device address `base`, its count word's address, the
+    slot's bytes); base None queries the size (null pointers)."""
+    out, count, size = capi.GrbLightList(), C.c_void_p(), C.c_uint64()
+    capi.check(capi.lib().grb_light_slot_layout(None if base is None else C.c_void_p(base), C.byref(out), C.byref(count), C.byref(size)),
+               "grb_light_slot_layout")
+    return out, count.value, size.value
+
+
+def light_list_to_peers(lights, input_count_t, slots, flag_arrays, flag_index, epoch, counter_t):
+    """grb_light_list_to_peers with every rank's slot and flag array as tensors on this device: lights a GrbLightList
+    (None with slots None), input_count_t a one-element int32 tensor or None, slots[r] a uint8 tensor of the slot's
+    bytes (None for every rank: a flags-only publish)."""
+    n = len(flag_arrays)
+    images = None if slots is None else (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_light_list_to_peers(None if lights is None else C.byref(lights), None if input_count_t is None else _ptr(input_count_t),
+                                                  images, flags, n, int(flag_index), int(epoch), _ptr(counter_t), capi.stream_ptr()),
+               "grb_light_list_to_peers")
+
+
 def to_dev(a):
     return _dev(a)
 

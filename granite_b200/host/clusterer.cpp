@@ -451,28 +451,34 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 		auto *type_mask = const_cast<uint32_t *>(buf.type_mask);
 		auto *z_ranges = const_cast<uint32_t *>(buf.z_ranges);
 		void *s = cmd.get_stream_handle();
+		GrbLightList list = src.list;
+		const int32_t *input_count = src.input_count;
+		if (src.exchange)
+			src.exchange(cmd, list, input_count);
 		if (enable_shadows)
 		{
 			// the shadow tables where the lighting pass reads them: packed_size(slots) and packed_offset_shadow_maps(slots)
 			const GrbLightShadows out = get_light_shadows();
 			auto *transforms = const_cast<float *>(out.transforms);
 			auto *maps = const_cast<const void **>(out.maps);
-			if (src.input_count)
-				cmd.check(grb_light_prep_shadowed_counted(&src.list, src.input_count, &src.shadows, &device_view, records, model, type_mask, z_ranges,
+			if (input_count)
+				cmd.check(grb_light_prep_shadowed_counted(&list, input_count, &src.shadows, &device_view, records, model, type_mask, z_ranges,
 				                                          transforms, maps, src.count, src.scratch, src.scratch_bytes, s),
 				          "grb_light_prep_shadowed_counted");
 			else
-				cmd.check(grb_light_prep_shadowed(&src.list, &src.shadows, &device_view, records, model, type_mask, z_ranges, transforms, maps, src.count,
+				cmd.check(grb_light_prep_shadowed(&list, &src.shadows, &device_view, records, model, type_mask, z_ranges, transforms, maps, src.count,
 				                                  src.scratch, src.scratch_bytes, s),
 				          "grb_light_prep_shadowed");
 		}
-		else if (src.input_count)
-			cmd.check(grb_light_prep_counted(&src.list, src.input_count, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch,
+		else if (input_count)
+			cmd.check(grb_light_prep_counted(&list, input_count, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch,
 			                                 src.scratch_bytes, s),
 			          "grb_light_prep_counted");
 		else
-			cmd.check(grb_light_prep(&src.list, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch, src.scratch_bytes, s),
+			cmd.check(grb_light_prep(&list, &device_view, records, model, type_mask, z_ranges, src.count, src.scratch, src.scratch_bytes, s),
 			          "grb_light_prep");
+		if (src.after_prep)
+			src.after_prep(cmd);
 		if (src.consumed)
 			Vulkan::cuda_ok(cudaEventRecord(static_cast<cudaEvent_t>(src.consumed), stream), "cudaEventRecord(lights consumed)");
 		launch_cluster_kernels(cmd, src.count, std::max<int32_t>(parameters.num_lights, 1));

@@ -5,6 +5,7 @@
 // decals, volumetrics of the reference's class are outside the hot path (SURVEY.md §2).
 #pragma once
 
+#include <functional>
 #include <memory>
 #include <vector>
 
@@ -99,11 +100,16 @@ public:
 	// `input_count` (device, or null = all list.count entries are lights) makes list.count a capacity: the prep
 	// (grb_light_prep[_shadowed]_counted) reads the live length under the same events; refresh() still sizes the frame
 	// from the capacity.
+	// Row-sharded frames whose list comes from one rank (scene_viewer.cpp, grbh_viewer_set_light_source_rank):
+	// `exchange` runs on the pass's stream after `ready` and may replace the list and count the prep reads with this
+	// frame's received copy; `after_prep` runs right behind the prep, before `consumed` and the cluster kernels.
 	struct DeviceLightSource
 	{
 		GrbLightList list = {};
 		GrbLightShadowList shadows = {};
 		const int32_t *input_count = nullptr;
+		std::function<void(Vulkan::CommandBuffer &, GrbLightList &, const int32_t *&)> exchange;
+		std::function<void(Vulkan::CommandBuffer &)> after_prep;
 		void *ready = nullptr, *consumed = nullptr;
 		void *scratch = nullptr; // grb_light_prep_scratch_bytes(list.count) or more
 		size_t scratch_bytes = 0;

@@ -196,6 +196,15 @@ bool NcclCollectives::all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, 
 	return collective_failed("all_reduce_sum_u32");
 }
 
+bool NcclCollectives::broadcast_bytes(Vulkan::Stream stream, void *data, size_t bytes, unsigned root)
+{
+	if (!comm || root >= world)
+		return false;
+	if (nccl_ok(api().Broadcast(data, data, bytes, ncclInt8, (int)root, comm, stream), "ncclBroadcast"))
+		return true;
+	return collective_failed("broadcast_bytes");
+}
+
 // ----------------------------------------------------------------------------- peer exchange
 void NcclCollectives::release_peer_exchange(PeerState &peer)
 {

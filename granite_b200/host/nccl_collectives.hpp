@@ -27,6 +27,7 @@ public:
 	bool all_gather_row_lists(Vulkan::CommandBuffer &cmd, Vulkan::ImageView &image, const std::vector<std::vector<GrbRows>> &rows) override;
 	bool all_reduce_sum(Vulkan::CommandBuffer &cmd, float *data, size_t count) override;
 	bool all_reduce_sum_u32(Vulkan::Stream stream, uint32_t *data, size_t count) override;
+	bool broadcast_bytes(Vulkan::Stream stream, void *data, size_t bytes, unsigned root) override;
 	// Peer-memory exchange: two image slots + a flag array per rank, cudaIpc-mapped into every
 	// other rank (handles are exchanged with one ncclAllGather).  GRB_SHARD_EXCHANGE=nccl disables it.
 	bool peer_exchange_begin_frame(PeerChannel channel, size_t image_bytes, PeerSlot &slot) override;
@@ -47,7 +48,7 @@ private:
 		std::vector<void *> opened;
 		uint32_t epoch = 0;
 	};
-	PeerState channels[(size_t)PeerChannel::GBuffer + 1]; // [PeerChannel]
+	PeerState channels[(size_t)PeerChannel::Lights + 1]; // [PeerChannel]
 	bool setup_peer_exchange(PeerState &channel, size_t image_bytes);
 	void release_peer_exchange(PeerState &channel);
 };

@@ -66,6 +66,16 @@ public:
 		(void)count;
 		return false;
 	}
+	// Broadcast of `bytes` bytes from rank `root` into `data` on every rank, in place on `stream`; false = not available.
+	// For the light channel without peer memory (scene_viewer.cpp, grbh_viewer_set_light_source_rank).
+	virtual bool broadcast_bytes(Vulkan::Stream stream, void *data, size_t bytes, unsigned root)
+	{
+		(void)stream;
+		(void)data;
+		(void)bytes;
+		(void)root;
+		return false;
+	}
 
 	// Peer-memory exchange: a double-buffered image every rank holds in full, of which each rank
 	// PRODUCES some rows per frame by storing them into all ranks' copies from its own kernel
@@ -86,6 +96,8 @@ public:
 		            // "lighting-exchange" passes of scene_viewer.cpp)
 		GBuffer,    // the G-buffer rows each rank reads, pushed by the one rank that rasterised the whole frame into every
 		            // other rank's slot (the "gbuffer" pass of scene_viewer.cpp under grbh_viewer_set_gbuffer_source_rank)
+		Lights,     // the live part of one rank's device light list, pushed into every other rank's slot by the clustering
+		            // pass (scene_viewer.cpp under grbh_viewer_set_light_source_rank)
 	};
 	struct PeerSlot
 	{

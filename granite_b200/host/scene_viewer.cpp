@@ -109,6 +109,17 @@ struct GrbhViewer
 	void *light_scratch = nullptr;
 	size_t light_scratch_bytes = 0;
 	bool device_prep_rendered = false;
+	// row-sharded frames whose device light list comes from one rank (-1: off; grbh_viewer_set_light_source_rank): that
+	// rank's clustering pass pushes the list's live entries into every other rank's slot of the light channel, and every
+	// other rank binds a receiving list (grbh_viewer_set_lights_device_from_source) whose prep reads its slot
+	int light_source = -1;
+	// the credit a receiving rank raises behind this frame's prep, when the list came through peer memory
+	bool light_credit_pending = false;
+	RenderGraphCollectives::PeerSlot light_credit;
+	// without peer memory: this rank's light slot (the source fills it, a broadcast carries it to every rank) and, past
+	// its end, the flag words and counter of the source's push; allocated on the first such frame
+	void *light_slot = nullptr;
+	uint32_t light_slot_epoch = 0;
 	std::vector<mat_affine> scene_decals;
 
 	mat4 projection = mat4(1.0f), view = mat4(1.0f);
@@ -202,6 +213,9 @@ struct GrbhViewer
 	std::string check_output_images(const GrbImage *images, int32_t count) const;
 	void set_output_ring(const GrbImage *images, int32_t count);
 	bool fed_from_source() const { return bands.size() > 1 && gbuffer_source >= 0; }
+	bool lights_from_source() const { return bands.size() > 1 && light_source >= 0; }
+	void exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count);
+	void raise_light_credit(Vulkan::CommandBuffer &cmd);
 
 	// the G-buffer planes of the attachments (grb_gbuffer_copy_rows order), the G-buffer ones and / or motion vectors
 	GrbGBufferPlanes attachment_planes(bool gbuffer_planes, bool mv)
@@ -330,6 +344,16 @@ void GrbhViewer::bake_render_graph()
 	else
 		cluster.set_lit_pixel_rows(0, 0, 0);
 	cluster.set_lit_tile_ranges(striped() ? stripe_plan().tile_rows : std::vector<GrbRows>{});
+	if (lights_from_source())
+	{
+		device_lights.exchange = [this](Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count) { exchange_lights(cmd, list, count); };
+		device_lights.after_prep = [this](Vulkan::CommandBuffer &cmd) { raise_light_credit(cmd); };
+	}
+	else
+	{
+		device_lights.exchange = nullptr;
+		device_lights.after_prep = nullptr;
+	}
 	cluster.add_render_passes(graph);
 	lighting.cluster = &cluster;
 	context.set_lighting_parameters(&lighting);
@@ -835,6 +859,85 @@ void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 			throw std::runtime_error("gbuffer: the broadcast of the G-buffer rows from the source rank failed");
 }
 
+// The light channel of a row-sharded frame whose device lights come from rank S (DESIGN.md section 5, "Lights from
+// device memory", "From one rank"), on the clustering pass's stream after the lights' `ready`.  Peer path: S waits for
+// every rank's credit of the last epoch and pushes its list's live entries into every rank's slot, then preps its own
+// list; every other rank waits for S's flag, preps its slot (the list and count returned here) and raises its credit
+// behind the prep (raise_light_credit).  Without peer memory: S fills its own slot with the same kernel and a broadcast
+// from S carries the whole slot into every rank's, in stream order with the prep that reads it.
+void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count)
+{
+	const unsigned S = (unsigned)light_source;
+	void *handle = cmd.get_stream_handle();
+	uint64_t bytes = 0;
+	if (!cmd.check(grb_light_slot_layout(nullptr, nullptr, nullptr, &bytes), "grb_light_slot_layout"))
+		return;
+	RenderGraphCollectives *coll = graph.get_collectives();
+	RenderGraphCollectives::PeerSlot slot;
+	void *received = nullptr;
+	if (coll->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::Lights, (size_t)bytes, slot))
+	{
+		if (rank == S)
+		{
+			// the credits: every rank's prep of the last epoch has read its slot, and by stream order the epoch's before
+			cmd.check(grb_peer_wait(slot.flags[S], (int32_t)slot.count, slot.epoch - 1u, handle), "grb_peer_wait");
+			cmd.check(grb_light_list_to_peers(&list, count, slot.images, slot.flags, (int32_t)slot.count, (int32_t)S, slot.epoch, slot.counter, handle),
+			          "grb_light_list_to_peers");
+			return;
+		}
+		cmd.check(grb_peer_wait(slot.flags[rank] + S, 1, slot.epoch, handle), "grb_peer_wait");
+		light_credit = slot;
+		light_credit_pending = true;
+		received = slot.images[rank];
+	}
+	else
+	{
+		if (!light_slot)
+		{
+			// zeroed on the pass's stream, ahead of the first push and broadcast (the push's counter must start at 0)
+			void *p = nullptr;
+			if (!Vulkan::cuda_ok(cudaMalloc(&p, (size_t)bytes + 256), "cudaMalloc(light slot)") ||
+			    !Vulkan::cuda_ok(cudaMemsetAsync(p, 0, (size_t)bytes + 256, cmd.get_stream()), "cudaMemsetAsync(light slot)"))
+			{
+				cudaFree(p);
+				throw std::runtime_error("clustering: allocating the light slot failed");
+			}
+			light_slot = p;
+		}
+		if (rank == S)
+		{
+			void *slots[1] = { light_slot };
+			uint32_t *flags[1] = { reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(light_slot) + bytes) };
+			cmd.check(grb_light_list_to_peers(&list, count, slots, flags, 1, 0, ++light_slot_epoch, flags[0] + 8, handle), "grb_light_list_to_peers");
+		}
+		if (!coll->broadcast_bytes(cmd.get_stream(), light_slot, (size_t)bytes, S))
+			throw std::runtime_error("clustering: the broadcast of the light list from the source rank failed");
+		if (rank == S)
+			return;
+		received = light_slot;
+	}
+	// this frame's slot as a list of this rank's own capacity: the prep clamps the pushed count to it
+	GrbLightList slot_list = {};
+	int32_t *slot_count = nullptr;
+	if (!cmd.check(grb_light_slot_layout(received, &slot_list, &slot_count, &bytes), "grb_light_slot_layout"))
+		return;
+	slot_list.count = list.count;
+	slot_list.cutoff_range = list.cutoff_range;
+	list = slot_list;
+	count = slot_count;
+}
+
+// A receiving rank's credit of the light channel: a flags-only publish behind the prep, the last read of its slot
+void GrbhViewer::raise_light_credit(Vulkan::CommandBuffer &cmd)
+{
+	if (!light_credit_pending)
+		return;
+	light_credit_pending = false;
+	cmd.check(grb_light_list_to_peers(nullptr, nullptr, nullptr, light_credit.flags, (int32_t)light_credit.count, (int32_t)rank, light_credit.epoch,
+	                                  light_credit.counter, cmd.get_stream_handle()),
+	          "grb_light_list_to_peers");
+}
+
 cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
 {
 	if (bands_moved)
@@ -1032,6 +1135,8 @@ extern "C" void grbh_viewer_destroy(GrbhViewer *viewer)
 	viewer->graph.reset();
 	if (viewer->light_scratch)
 		cudaFree(viewer->light_scratch);
+	if (viewer->light_slot)
+		cudaFree(viewer->light_slot);
 	if (viewer->device)
 		Granite::release_smaa_lookup_textures(*viewer->device); // device images: must go before the device does
 	delete viewer;
@@ -1189,6 +1294,15 @@ int32_t bind_device_lights(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhD
 	v->device_prep_rendered = false;
 	return 0;
 }
+
+// "" unless the device light list of this rank comes from another rank (grbh_viewer_set_light_source_rank)
+std::string not_light_source(const GrbhViewer *v)
+{
+	if (v->light_source < 0 || v->rank == (unsigned)v->light_source)
+		return "";
+	return "rank " + std::to_string(v->rank) + " receives its device lights from light source rank " + std::to_string(v->light_source) +
+	       " (grbh_viewer_set_light_source_rank); it binds grbh_viewer_set_lights_device_from_source";
+}
 } // namespace
 
 extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDeviceLights *l)
@@ -1201,6 +1315,9 @@ extern "C" int32_t grbh_viewer_set_lights_device(GrbhViewer *v, const GrbhDevice
 	if (v->config.clustered_lights_shadows)
 		return fail(fn + "the viewer was created with clustered_lights_shadows; its device lights need their shadows "
 		                 "(grbh_viewer_set_lights_device_shadowed)");
+	const std::string receiver = not_light_source(v);
+	if (!receiver.empty())
+		return fail(fn + receiver);
 	if (!v->device)
 		return fail(fn + "host-only viewer (no CUDA device)");
 	GRBH_TRY
@@ -1231,6 +1348,9 @@ extern "C" int32_t grbh_viewer_set_light_count_device(GrbhViewer *v, const int32
 	const std::string fn = "grbh_viewer_set_light_count_device: ";
 	if (!v)
 		return fail(fn + "null viewer");
+	const std::string receiver = not_light_source(v);
+	if (!receiver.empty())
+		return fail(fn + receiver + ", whose count comes with the list");
 	if (!v->device)
 		return fail(fn + "host-only viewer (no CUDA device)");
 	if (!v->cluster.has_device_lights())
@@ -1245,6 +1365,32 @@ extern "C" int32_t grbh_viewer_set_light_count_device(GrbhViewer *v, const int32
 			return -1;
 	}
 	v->device_lights.input_count = count;
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_lights_device_from_source(GrbhViewer *v, int32_t capacity, float cutoff_range)
+{
+	const std::string fn = "grbh_viewer_set_lights_device_from_source: ";
+	if (!v)
+		return fail(fn + "null viewer");
+	if (v->light_source < 0)
+		return fail(fn + "the viewer has no light source rank (grbh_viewer_set_light_source_rank)");
+	if (v->rank == (unsigned)v->light_source)
+		return fail(fn + "rank " + std::to_string(v->rank) + " is the light source rank; it binds its list with grbh_viewer_set_lights_device");
+	if (capacity < 0 || capacity > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(fn + "capacity " + std::to_string(capacity) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	GRBH_TRY
+	// a list with no arrays of its own: every frame's clustering pass points the prep at the slot the source filled
+	GrbhDeviceLights none = {};
+	none.count = 0;
+	none.cutoff_range = cutoff_range;
+	const int32_t rc = bind_device_lights(v, &none, nullptr, fn);
+	if (rc != 0)
+		return rc;
+	v->device_lights.list.count = capacity;
 	return 0;
 	GRBH_CATCH
 }
@@ -1377,6 +1523,9 @@ extern "C" int32_t grbh_viewer_set_row_shards(GrbhViewer *v, const GrbRows *band
 	if (v->gbuffer_source >= std::max(count, 1))
 		return fail("grbh_viewer_set_row_shards: the G-buffer source rank " + std::to_string(v->gbuffer_source) + " would have no band among " +
 		            std::to_string(count) + " (call grbh_viewer_set_gbuffer_source_rank first)");
+	if (v->light_source >= std::max(count, 1))
+		return fail("grbh_viewer_set_row_shards: the light source rank " + std::to_string(v->light_source) + " would have no band among " +
+		            std::to_string(count) + " (call grbh_viewer_set_light_source_rank first)");
 	v->bands.assign(bands, bands + count);
 	v->rank = (unsigned)rank;
 	v->baked = false;
@@ -1409,6 +1558,22 @@ extern "C" int32_t grbh_viewer_set_gbuffer_source_rank(GrbhViewer *v, int32_t ra
 		return fail("grbh_viewer_set_gbuffer_source_rank: not with pipelined_io (the G-buffer channel already keeps two slots in flight)");
 	v->gbuffer_source = rank;
 	v->baked = false;
+	return 0;
+}
+
+extern "C" int32_t grbh_viewer_set_light_source_rank(GrbhViewer *v, int32_t rank)
+{
+	const std::string fn = "grbh_viewer_set_light_source_rank: ";
+	if (!v)
+		return fail(fn + "null viewer");
+	if (rank >= 0 && v->config.clustered_lights_shadows)
+		return fail(fn + "not with clustered_lights_shadows (a light's shadow map pointer is valid on its own rank only)");
+	const int32_t count = std::max((int32_t)v->bands.size(), 1); // an unsharded viewer is one band
+	if (rank < -1 || rank >= count)
+		return fail(fn + "rank must be -1 (off) or within [0, " + std::to_string(count) + ") (the bands of the last grbh_viewer_set_row_shards)");
+	if (v->baked)
+		return fail(fn + "the viewer is baked; set the light source rank before grbh_viewer_bake");
+	v->light_source = rank;
 	return 0;
 }
 

@@ -77,6 +77,7 @@ def lib() -> C.CDLL:
         _lib.grbh_viewer_set_output_images.argtypes = [C.c_void_p, C.c_void_p, C.c_int32]
         _lib.grbh_viewer_acquire_output.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         _lib.grbh_viewer_set_light_count_device.argtypes = [C.c_void_p, C.c_void_p]
+        _lib.grbh_viewer_set_lights_device_from_source.argtypes = [C.c_void_p, C.c_int32, C.c_float]
     return _lib
 
 
@@ -503,6 +504,21 @@ class Viewer:
         render_frame_device every frame, that rank with the whole G-buffer and every other rank with None.  Every rank
         sets the same value, before bake; not with pipelined_io (grbh_viewer_set_gbuffer_source_rank)."""
         _check(lib().grbh_viewer_set_gbuffer_source_rank(self._h, int(rank)), "grbh_viewer_set_gbuffer_source_rank")
+
+    def set_light_source_rank(self, rank):
+        """Row-sharded frames whose device light list comes from `rank` (-1: off): that rank binds its list (and count)
+        with set_lights_device, every other rank calls set_lights_device_from_source with the same capacity and cutoff
+        between the same two frames, and each frame pushes the list's live entries and count from that rank into every
+        other rank's clustering pass.  Every rank sets the same value, before bake; not with light_shadows
+        (grbh_viewer_set_light_source_rank)."""
+        _check(lib().grbh_viewer_set_light_source_rank(self._h, int(rank)), "grbh_viewer_set_light_source_rank")
+
+    def set_lights_device_from_source(self, capacity, cutoff=1e10):
+        """The receiving binding of a rank other than the light source rank: frames prep the list the source rank pushes,
+        as a list of `capacity` entries (the source's set_lights_device length) with `cutoff`
+        (grbh_viewer_set_lights_device_from_source).  Until the next set_lights[_device*] call."""
+        _check(lib().grbh_viewer_set_lights_device_from_source(self._h, int(capacity), float(cutoff)), "grbh_viewer_set_lights_device_from_source")
+        self._device_lights = ()
 
     def input_rows(self):
         """The (y0, y1) row ranges of the render-size G-buffer this rank reads: the rows a sort-first rasteriser on this

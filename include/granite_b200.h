@@ -235,6 +235,30 @@ int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, const int32_
                                         const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges,
                                         float *shadow_transforms_out, const void **shadow_maps_out, int32_t *device_count, void *scratch,
                                         uint64_t scratch_bytes, void *stream);
+/* The largest light list the prep takes (GRBH_MAX_DEVICE_LIGHTS of the host API). */
+#define GRB_MAX_LIGHT_LIST 65536
+/* The light slot of a row-sharded frame's light channel: a GrbLightList of GRB_MAX_LIGHT_LIST entries plus the count
+ * word that grb_light_list_to_peers stores the pushed length in -- the count word at the slot's start, then color,
+ * position, is_point, rotation, inner_cone and outer_cone, each from a multiple of 256 bytes (about 4.5 MB in all).
+ * *bytes receives the slot's size.  slot (16-byte aligned) may be NULL to query the size only; out and count_out (may
+ * be NULL) then receive NULL pointers.  out->count = GRB_MAX_LIGHT_LIST and out->cutoff_range = 0: a receiver sets its
+ * own capacity and cutoff.  GRB_ERR_INVALID_ARGUMENT: a null `bytes`, a slot that is not 16-byte aligned. */
+int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t **count_out, uint64_t *bytes);
+/* Pushing one rank's device light list to every rank of a row-sharded frame: reads live = min(max(*input_count, 0),
+ * lights->count) on the device (live = lights->count when input_count is NULL), stores bytes [0, live x element size)
+ * of each of the six arrays into the same array of every peer_slots[r] (the base address, valid on this device, of
+ * rank r's slot: cudaIpc-mapped peer memory, or local memory; the layout of grb_light_slot_layout) and live into the
+ * slot's count word.  No entry at or past live is read.  16-byte loads and stores where the array and every slot are
+ * 16-byte aligned, 4-byte ones for the float arrays where they are 4-byte aligned, bytes otherwise.  Then flags[flag_index] =
+ * epoch is release-stored into the flag array of EVERY rank.  The grid is sized from the capacity (lights->count):
+ * the length is not known on the host.  peer_slots may be NULL: a flags-only publish (the credit a receiving rank
+ * raises once its prep has read its slot), for which lights and input_count may be NULL.  scratch_counter: one
+ * zero-initialised uint32 in local device memory.  GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside
+ * 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, a count outside 0..GRB_MAX_LIGHT_LIST, an input count that is not
+ * 4-byte aligned, a slot that is not 16-byte aligned (checked before any CUDA call; nothing is written).  No reference
+ * equivalent (the reference never splits a frame). */
+int32_t grb_light_list_to_peers(const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
+                                int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream);
 
 /* Volumetric-decal binning over the clusterer's tile grid: LightClusterer::update_bindless_mask_buffer_decal_gpu
  * (clusterer.cpp:1391-1461) + clusterer_bindless_binning_decal.comp.  mvps: num_decals x mat4 (column-major, device) =

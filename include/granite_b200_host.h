@@ -156,7 +156,8 @@ int32_t grbh_viewer_set_lights(GrbhViewer *viewer, const GrbhLights *lights);
  * the host prep of the same lights gives, and the kept count never comes back to the host.  The arrays must be device
  * memory of the viewer's device and stay alive while frames that read them are in flight.  Refused: a host-only viewer,
  * a count outside 0..GRBH_MAX_DEVICE_LIGHTS, a viewer created with clustered_lights_shadows (whose device lights go
- * through grbh_viewer_set_lights_device_shadowed). */
+ * through grbh_viewer_set_lights_device_shadowed), a rank other than the light source rank of
+ * grbh_viewer_set_light_source_rank. */
 int32_t grbh_viewer_set_lights_device(GrbhViewer *viewer, const GrbhDeviceLights *lights);
 /* grbh_viewer_set_lights_device for a viewer created with clustered_lights_shadows: the clustering pass also moves each
  * kept light's shadow transform and map pointer into cluster order, so frames equal those of host lights given the same
@@ -171,7 +172,9 @@ int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *viewer, const GrbhDev
  * (a value written on the device cannot be refused, so it is clamped); entries [live, capacity) are never read.  The
  * frame equals the frame of the first `live` lights bound without a count.  count: device memory of the viewer's device,
  * 4-byte aligned, alive while frames that read it are in flight; NULL goes back to every bound entry being live.
- * grbh_viewer_set_lights[_device[_shadowed]] clear it: a new binding is a new list.  Refused: a null viewer, a host-only
+ * grbh_viewer_set_lights[_device[_shadowed]] clear it: a new binding is a new list.  On a row-sharded viewer with a
+ * light source rank (grbh_viewer_set_light_source_rank) the count goes with the list to every other rank, so the ranks
+ * need no copies of it to keep equal.  Refused: a null viewer, a rank other than the light source rank, a host-only
  * viewer, no device light list bound, a count that is not 4-byte aligned or not device memory of the viewer's device. */
 int32_t grbh_viewer_set_light_count_device(GrbhViewer *viewer, const int32_t *count);
 int32_t grbh_viewer_set_exposure(GrbhViewer *viewer, float exposure);
@@ -245,6 +248,27 @@ int32_t grbh_viewer_move_row_shards(GrbhViewer *viewer, const GrbRows *bands, in
  * frame from one rank"); without peer memory the rows go out in NCCL broadcasts.  Call before bake, with the same value
  * on every rank.  Refused with pipelined_io. */
 int32_t grbh_viewer_set_gbuffer_source_rank(GrbhViewer *viewer, int32_t rank);
+/* Row-sharded frames whose device light list comes from one rank: rank -1 = off (the default), otherwise within [0, band
+ * count) of the last grbh_viewer_set_row_shards (an unsharded viewer counts as one band: it accepts 0, and that changes
+ * nothing).  That rank S binds its list as today (grbh_viewer_set_lights_device, grbh_viewer_set_light_count_device);
+ * every other rank binds a receiving list (grbh_viewer_set_lights_device_from_source), and both are refused on the
+ * ranks they do not belong to.  Every frame S's clustering pass, after the lights' `ready`, pushes the list's live
+ * entries and its live count into every other rank's slot of a double-buffered light channel (through NVLink peer
+ * memory, or a broadcast of the whole slot without it), then preps its own list; every other rank preps its slot with
+ * the counted prep.  So every rank renders the same list and the same count from one binding, with no host read of the
+ * count (DESIGN.md section 5, "Lights from device memory").
+ * Collective contract: every rank sets the same value before bake.  Every binding on S (with or without a count) is
+ * matched by a receiving binding of the same capacity and cutoff on every other rank, between the same two frames;
+ * grbh_viewer_set_lights (host lights) is called on every rank or on none.  Refused: a viewer created with
+ * clustered_lights_shadows (a light's shadow map pointer is only valid on its own rank), a rank out of range, a call
+ * after bake. */
+int32_t grbh_viewer_set_light_source_rank(GrbhViewer *viewer, int32_t rank);
+/* The receiving binding of a rank other than the light source rank: from the next frame, the clustering pass preps the
+ * list the source rank pushed this frame, as a list of `capacity` entries with cutoff_range, so the frame is sized from
+ * `capacity` exactly as on the source rank.  The pushed count is clamped to `capacity`.  grbh_viewer_get_light_prep
+ * reads this rank's own prep.  Refused: a null viewer, a viewer with no light source rank, the light source rank itself,
+ * a capacity outside 0..GRBH_MAX_DEVICE_LIGHTS, a host-only viewer. */
+int32_t grbh_viewer_set_lights_device_from_source(GrbhViewer *viewer, int32_t capacity, float cutoff_range);
 /* The row ranges of the render-size G-buffer this rank reads: its lighting rows (grbh_shard_plan*), or the upload list
  * of grbh_shard_plan_stripes under lighting in stripes; {0, render height} unsharded.  These are the rows a sort-first
  * rasteriser on this rank must produce: a device G-buffer needs only these rows to be valid.  Returns the count;

@@ -7,7 +7,7 @@ moved every frame by a small torch op on the device, by where the light prep run
   on the GPU.
 
     python tools/device_lights_times.py [--frames 100] [--shadows | --live-count]
-    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows | --live-count]
+    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows | --live-count [--source-rank]]
 
 --shadows: viewers created with clustered_lights_shadows, every light shadowed by one of 64 static synthetic cube maps
 (64 x 64 texels a face).  Host lights get the map pointers with set_lights every frame and the clusterer computes the
@@ -24,6 +24,17 @@ Three ways to hand that list over are timed in the same run:
 - "parked": no compaction: the whole capacity is bound and dead particles are parked behind the camera, where the
   frustum cull drops them.
 The torch ops run on the caller's stream and the viewer waits on them through the lights' ready / consumed events.
+
+--live-count --source-rank (under torchrun): the same particle workload on row-sharded frames, with three hand-overs of
+the list from the rank that simulates it:
+- "every rank updates": every rank runs the particle update and the compaction on its own copy and binds its own list
+  and count (what a caller does without a source rank);
+- "caller broadcast": rank 0 updates and compacts; every frame the caller broadcasts the capacity-sized list and the
+  count from rank 0 (torch.distributed.broadcast on its stream, between the lights' ready / consumed events), and every
+  rank binds its copy once;
+- "viewer push": rank 0 updates, compacts and binds once; every other rank binds a receiving list once
+  (set_light_source_rank(0), set_lights_device_from_source), and rank 0's clustering pass pushes the live entries and
+  the count to the other ranks.
 
 Two light lists: 4096 input lights (all in view), and 16384 input lights of which 4096 are kept.  Under torchrun, one
 rank per GPU, row-sharded frames with every rank binding its own copy of the lights; the sharded rate is that of the
@@ -99,8 +110,10 @@ def particles():
     return lights, cycle, lifetime, offset
 
 
-def live_count_stepper(mode, lights, cycle, lifetime, offset):
-    """step(v, i) for one --live-count mode: the particle update, the compaction (or the parking) and the frame."""
+def live_count_stepper(mode, lights, cycle, lifetime, offset, rank=0):
+    """step(v, i) for one --live-count mode: the particle update, the compaction (or the parking) and the frame.  The
+    --source-rank modes: "every rank updates" is "device count" on every rank; under "caller broadcast" and "viewer
+    push" only rank 0 updates."""
     n = PARTICLES
     src = cases.to_device(lights)
     cycle_t, lifetime_t, offset_t = (torch.from_numpy(a).cuda() for a in (cycle, lifetime, offset))
@@ -112,16 +125,30 @@ def live_count_stepper(mode, lights, cycle, lifetime, offset):
     ready, consumed = torch.cuda.Event(), torch.cuda.Event()
     state = {"viewer": None}
 
+    receiver = mode in ("caller broadcast", "viewer push") and rank != 0
+
     def step(v, i):
         if state["viewer"] is not v:
             state["viewer"] = v
             state["gbs"] = [v.device_gbuffer(*g) for g in state["dev"]]
-            if mode == "device count":
+            if mode == "viewer push" and receiver:
+                v.set_lights_device_from_source(n)
+            elif mode in ("device count", "every rank updates", "caller broadcast", "viewer push"):
                 v.set_lights_device(**bound, ready=ready, consumed=consumed, count=count)
             elif mode == "parked":
                 v.set_lights_device(**parked, ready=ready, consumed=consumed)
         else:
             torch.cuda.current_stream().wait_event(consumed)
+        if mode == "viewer push" and receiver:
+            v.render_frame_device(state["gbs"][i % 2])
+            return
+        if receiver:
+            # the caller's broadcast of the capacity: the live length is only on the device
+            for t in (*bound.values(), count):
+                torch.distributed.broadcast(t, 0)
+            ready.record()
+            v.render_frame_device(state["gbs"][i % 2])
+            return
         alive = (i + offset_t) % cycle_t < lifetime_t
         if mode == "parked":
             for k in parked:
@@ -133,6 +160,9 @@ def live_count_stepper(mode, lights, cycle, lifetime, offset):
             for k in out:
                 out[k].index_copy_(0, dest, src[k])
             count.copy_(csum[-1:])
+        if mode == "caller broadcast":
+            for t in (*bound.values(), count):
+                torch.distributed.broadcast(t, 0)
         ready.record()
         if mode == "count read back":
             k = int(count.item())
@@ -142,17 +172,38 @@ def live_count_stepper(mode, lights, cycle, lifetime, offset):
     return step, state
 
 
+def source_rank_viewer(scene, bands, **config):
+    """sharded.make_viewer's row-sharded viewer with light source rank 0, which must be set before bake (collective)."""
+    v = viewer.Viewer(W, H, cuda_device=torch.cuda.current_device(), **config)
+    v.set_directional(scene.dir_color, scene.dir_direction)
+    rank = torch.distributed.get_rank()
+    uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
+    if rank == 0:
+        uid.copy_(torch.frombuffer(bytearray(viewer.nccl_unique_id()), dtype=torch.uint8))
+    torch.distributed.broadcast(uid, 0)
+    v.init_collectives(uid.cpu().numpy().tobytes(), rank, torch.distributed.get_world_size())
+    v.set_row_shards(bands, rank)
+    v.set_light_source_rank(0)
+    v.set_camera(scene.projection, scene.view)
+    v.bake()
+    return v
+
+
 def live_count_runs(args, scene, dev, bands, card, distributed, rank, world):
     lights, cycle, lifetime, offset = particles()
     closer = sharded.close_sharded if distributed else (lambda v: v.close())
     runs = []
-    for mode in ("device count", "count read back", "parked"):
+    modes = ("every rank updates", "caller broadcast", "viewer push") if args.source_rank else ("device count", "count read back", "parked")
+    for mode in modes:
         times = []
         for timestamps in (False, True):
-            step, state = live_count_stepper(mode, lights, cycle, lifetime, offset)
+            step, state = live_count_stepper(mode, lights, cycle, lifetime, offset, rank)
             state["dev"] = dev
             stream = torch.cuda.Stream()
-            v = sharded.make_viewer(W, H, scene, synth.make_lights(0), scene.view, bands=bands, stream=stream.cuda_stream, timestamps=timestamps)
+            if mode == "viewer push":
+                v = source_rank_viewer(scene, bands, stream=stream.cuda_stream, timestamps=timestamps)
+            else:
+                v = sharded.make_viewer(W, H, scene, synth.make_lights(0), scene.view, bands=bands, stream=stream.cuda_stream, timestamps=timestamps)
             times.append(timed(v, stream, args.frames, step))
             if timestamps:
                 t, c = v.collect_timings().get("clustering-bindless", (0.0, 0))
@@ -198,10 +249,13 @@ def main():
     ap.add_argument("--frames", type=int, default=100)
     ap.add_argument("--shadows", action="store_true", help="shadowed lights with static synthetic maps")
     ap.add_argument("--live-count", action="store_true", help="a compacted particle list whose length is known only on the device")
+    ap.add_argument("--source-rank", action="store_true", help="with --live-count under torchrun: hand the list over from rank 0")
     args = ap.parse_args()
     if args.shadows and args.live_count:
         ap.error("--shadows and --live-count are separate workloads")
     distributed = "RANK" in os.environ
+    if args.source_rank and not (args.live_count and distributed):
+        ap.error("--source-rank times the --live-count workload on row-sharded frames: run it with --live-count under torchrun")
     if distributed:
         rank, world, local = sharded.init_ranks(allow_shared=False)
     else:
@@ -216,7 +270,7 @@ def main():
               "frames_timed": args.frames, "fill_frames": FILL, "ranks": world, "gpu": card, "runs": []}
     if args.live_count:
         result["workload"] = (f"c3: 3840x2160, bloom + tonemap, device G-buffer every frame, {PARTICLES} particle lights of which about half "
-                              "are alive, compacted on the device every frame")
+                              "are alive, compacted on the device every frame" + (", handed over from rank 0" if args.source_rank else ""))
         result["runs"] = live_count_runs(args, scene, dev, bands, card, distributed, rank, world)
         if rank == 0:
             print(json.dumps(result), flush=True)
