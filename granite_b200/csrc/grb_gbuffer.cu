@@ -325,7 +325,7 @@ extern "C" int32_t grb_gbuffer_rows_to_peers(const GrbGBufferPlanes *src, void *
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	PeerTargets targets;
-	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets, /*flags_only=*/peer_slots == nullptr))
+	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
 		return GRB_ERR_INVALID_ARGUMENT;
 	unsigned present = 0;
 	int w = 0, h = 0;
@@ -342,16 +342,16 @@ extern "C" int32_t grb_gbuffer_rows_to_peers(const GrbGBufferPlanes *src, void *
 		}
 		total += range_counts[q];
 	}
-	if (total > 0 && (!rows || !peer_slots))
+	if (total > 0 && !rows)
 	{
-		fail_arg(fn, "rows to copy need the row list and the peers' slots (a flags-only publish lists no rows)");
+		fail_arg(fn, "rows to copy need the row list");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	uint64_t offsets[kPlanes];
 	slot_offsets(src, offsets);
 	PlaneArgs planes = {};
 	bool slots16 = true;
-	for (int q = 0; peer_slots && q < peer_count; q++)
+	for (int q = 0; q < peer_count; q++)
 		slots16 = slots16 && aligned16(peer_slots[q]);
 	for (int p = 0; p < kPlanes; p++)
 	{

@@ -105,21 +105,17 @@ __global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights,
 		*count_out = count;
 }
 
-// One thread per 16-byte chunk of the capacity's six arrays (lp::push_light_chunk), then the count word and the
-// publish.  No slots: a flags-only publish.
+// One thread per 16-byte chunk of the capacity's six arrays (lp::push_light_chunk), then the count word and the publish.
 __global__ void __launch_bounds__(256) light_push_kernel(lp::LightPush push, const int32_t *__restrict__ input_count, int capacity, PeerTargets targets)
 {
-	if (targets.data[0])
-	{
-		const int live = input_count ? lp::live_count(*input_count, capacity) : capacity;
-		const int t = blockIdx.x * blockDim.x + threadIdx.x;
-		lp::push_light_chunk(push, live, t, targets.data, targets.count);
-		if (t == 0)
+	const int live = input_count ? lp::live_count(*input_count, capacity) : capacity;
+	const int t = blockIdx.x * blockDim.x + threadIdx.x;
+	lp::push_light_chunk(push, live, t, targets.data, targets.count);
+	if (t == 0)
 #pragma unroll
-			for (int r = 0; r < GRB_MAX_PEERS; r++)
-				if (r < targets.count)
-					*reinterpret_cast<int32_t *>(static_cast<uint8_t *>(targets.data[r]) + lp::light_slot_layout().count) = live;
-	}
+		for (int r = 0; r < GRB_MAX_PEERS; r++)
+			if (r < targets.count)
+				*reinterpret_cast<int32_t *>(static_cast<uint8_t *>(targets.data[r]) + lp::light_slot_layout().count) = live;
 	peer_publish(targets);
 }
 
@@ -312,13 +308,8 @@ extern "C" int32_t grb_light_list_to_peers(const GrbLightList *lights, const int
 {
 	const char *fn = "grb_light_list_to_peers";
 	PeerTargets targets;
-	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets, /*flags_only=*/peer_slots == nullptr))
+	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
 		return GRB_ERR_INVALID_ARGUMENT;
-	if (!peer_slots)
-	{
-		light_push_kernel<<<1, 256, 0, as_stream(stream)>>>(lp::LightPush{}, nullptr, 0, targets);
-		return check_launch(fn);
-	}
 	if (!lights || lights->count < 0 || lights->count > GRB_MAX_LIGHT_LIST ||
 	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone || !lights->outer_cone)))
 	{

@@ -85,8 +85,8 @@ inline unsigned peer_wait_max_spins()
 
 // Checks the peer arguments of entry point `fn` and fills `t`; false (with the message set) on a bad argument.
 // `flags_only`: no `images` (NULL) -- the kernel writes one rank's slot, which its caller passes on its own
-// (grb_present_rows_to_peer).  flag_index must name one of the flag words the ranks wait on: a word past them may hold
-// the scratch counter.
+// (grb_present_rows_to_peer), or none (grb_peer_publish).  flag_index must name one of the flag words the ranks wait
+// on: a word past them may hold the scratch counter.
 inline bool peer_targets_from(const char *fn, void *const *images, uint32_t *const *flags, int32_t count, int32_t flag_index, uint32_t epoch,
                               uint32_t *counter, PeerTargets &t, bool flags_only = false)
 {

@@ -149,6 +149,9 @@ __global__ void peer_wait_kernel(const uint32_t *flags, int count, uint32_t epoc
 		peer_wait(flags, threadIdx.x, epoch, error_word, max_spins);
 }
 
+// A publish with no slot data: the credit a receiving rank raises behind its last read of a slot.
+__global__ void peer_publish_kernel(PeerTargets targets) { peer_publish(targets); }
+
 // Presenting a row-sharded frame from one rank: each rank copies its band of the final 4-byte-per-texel image into the
 // presenting rank's frame slot (IPC-mapped peer memory over NVLink; a local copy on the presenting rank itself), then
 // publishes "band of frame <epoch> landed" in every rank's flag array (grb_peer.cuh).
@@ -1040,6 +1043,16 @@ extern "C" int32_t grb_peer_wait(const uint32_t *local_flags, int32_t count, uin
 	}
 	peer_wait_kernel<<<1, 32, 0, as_stream(stream)>>>(local_flags, count, epoch, device_error_word(), peer_wait_max_spins());
 	return check_launch("grb_peer_wait");
+}
+
+extern "C" int32_t grb_peer_publish(uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter,
+                                    void *stream)
+{
+	PeerTargets targets;
+	if (!peer_targets_from("grb_peer_publish", nullptr, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets, /*flags_only=*/true))
+		return GRB_ERR_INVALID_ARGUMENT;
+	peer_publish_kernel<<<1, 32, 0, as_stream(stream)>>>(targets);
+	return check_launch("grb_peer_publish");
 }
 
 static int texel_bytes(int32_t format)

@@ -358,6 +358,14 @@ def taa_resolve_to_peers(hdr_t, depth_t, mv_t, history_t, reproj, quality, out_c
                "grb_taa_resolve_to_peers")
 
 
+def peer_publish(flag_arrays, flag_index, epoch, counter_t):
+    """grb_peer_publish with every rank's flag array as tensors on this device: flag_arrays[r] an int32 tensor;
+    counter_t: one zeroed int32."""
+    flags = (C.c_void_p * len(flag_arrays))(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_peer_publish(flags, len(flag_arrays), int(flag_index), int(epoch), _ptr(counter_t), capi.stream_ptr()),
+               "grb_peer_publish")
+
+
 def present_rows_to_peer(src_t, dst_t, flag_arrays, flag_index, epoch, counter_t, own, fmt=capi.FORMAT_R8G8B8A8_SRGB, width=None):
     """grb_present_rows_to_peer with the presenting rank's slot and every rank's flag array as tensors on this device:
     src_t / dst_t: (H, P) int32 (one 4-byte texel each; the image is the first `width` texels of each row, all P by
@@ -396,12 +404,12 @@ def gbuffer_slot_layout(layout, base=None):
 
 def gbuffer_rows_to_peers(src, slots, flag_arrays, rows_per_rank, flag_index, epoch, counter_t):
     """grb_gbuffer_rows_to_peers with every rank's slot and flag array as tensors on this device: slots[q] a uint8
-    tensor of the slot's bytes (None for every rank: a flags-only publish), rows_per_rank[q] rank q's (y0, y1) list."""
+    tensor of the slot's bytes, rows_per_rank[q] rank q's (y0, y1) list."""
     n = len(flag_arrays)
     flat = [r for lst in rows_per_rank for r in lst]
     rs = (capi.GrbRows * max(len(flat), 1))(*[capi.GrbRows(int(a), int(b)) for a, b in flat])
     counts = (C.c_int32 * n)(*[len(lst) for lst in rows_per_rank])
-    images = None if slots is None else (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in slots])
     flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
     capi.check(capi.lib().grb_gbuffer_rows_to_peers(C.byref(src), images, flags, rs, counts, n, int(flag_index), int(epoch), _ptr(counter_t),
                                                     capi.stream_ptr()),
@@ -425,14 +433,13 @@ def light_slot_layout(base=None):
 
 
 def light_list_to_peers(lights, input_count_t, slots, flag_arrays, flag_index, epoch, counter_t):
-    """grb_light_list_to_peers with every rank's slot and flag array as tensors on this device: lights a GrbLightList
-    (None with slots None), input_count_t a one-element int32 tensor or None, slots[r] a uint8 tensor of the slot's
-    bytes (None for every rank: a flags-only publish)."""
+    """grb_light_list_to_peers with every rank's slot and flag array as tensors on this device: lights a GrbLightList,
+    input_count_t a one-element int32 tensor or None, slots[r] a uint8 tensor of the slot's bytes."""
     n = len(flag_arrays)
-    images = None if slots is None else (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in slots])
     flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
-    capi.check(capi.lib().grb_light_list_to_peers(None if lights is None else C.byref(lights), None if input_count_t is None else _ptr(input_count_t),
-                                                  images, flags, n, int(flag_index), int(epoch), _ptr(counter_t), capi.stream_ptr()),
+    capi.check(capi.lib().grb_light_list_to_peers(C.byref(lights), _ptr(input_count_t), images, flags, n, int(flag_index), int(epoch), _ptr(counter_t),
+                                                  capi.stream_ptr()),
                "grb_light_list_to_peers")
 
 

@@ -88,9 +88,39 @@ struct GrbhViewer
 		bool peer = false;
 		RenderGraphCollectives::PeerSlot slot;
 	} stripe_exchange;
+	// A peer channel that one source rank S fills for every rank, with credits (DESIGN.md section 5, "Feeding a sharded
+	// frame from one rank")
+	struct SourceHandover
+	{
+		RenderGraphCollectives::PeerChannel channel;
+		RenderGraphCollectives::PeerSlot slot;
+		bool credit_owed = false;
+		// Peer memory: S waits for every rank's credit of the last epoch (the last read of every slot, by stream order);
+		// any other rank waits for S's flag of this epoch and owes a credit.  false: no peer memory (the caller's NCCL path).
+		bool begin(Vulkan::CommandBuffer &cmd, RenderGraphCollectives &coll, size_t bytes, unsigned source, unsigned rank)
+		{
+			credit_owed = false;
+			if (!coll.peer_exchange_begin_frame(channel, bytes, slot))
+				return false;
+			credit_owed = rank != source;
+			if (credit_owed)
+				cmd.check(grb_peer_wait(slot.flags[rank] + source, 1, slot.epoch, cmd.get_stream_handle()), "grb_peer_wait");
+			else
+				cmd.check(grb_peer_wait(slot.flags[source], (int32_t)slot.count, slot.epoch - 1u, cmd.get_stream_handle()), "grb_peer_wait");
+			return true;
+		}
+		// A receiving rank, behind its last read of slot.images[rank]: grb_peer_publish.  No-op when no credit is owed.
+		void credit(Vulkan::CommandBuffer &cmd, unsigned rank)
+		{
+			if (credit_owed)
+				cmd.check(grb_peer_publish(slot.flags, (int32_t)slot.count, (int32_t)rank, slot.epoch, slot.counter, cmd.get_stream_handle()), "grb_peer_publish");
+			credit_owed = false;
+		}
+	};
 	// row-sharded frames fed from the one rank that rasterises the whole frame (-1: off;
 	// grbh_viewer_set_gbuffer_source_rank): its "gbuffer" pass pushes every rank's input rows into that rank's slot
 	int gbuffer_source = -1;
+	SourceHandover gbuffer_handover{ RenderGraphCollectives::PeerChannel::GBuffer };
 	// the caller's ring of output images (grbh_viewer_set_output_images), wrapped once each for the ring's life (the
 	// graph's cross-stream tracking keys on the wrapper), and the image, events of the next frame's acquire (-1: none)
 	std::vector<std::unique_ptr<Vulkan::ImageView>> output_ring;
@@ -113,9 +143,7 @@ struct GrbhViewer
 	// rank's clustering pass pushes the list's live entries into every other rank's slot of the light channel, and every
 	// other rank binds a receiving list (grbh_viewer_set_lights_device_from_source) whose prep reads its slot
 	int light_source = -1;
-	// the credit a receiving rank raises behind this frame's prep, when the list came through peer memory
-	bool light_credit_pending = false;
-	RenderGraphCollectives::PeerSlot light_credit;
+	SourceHandover light_handover{ RenderGraphCollectives::PeerChannel::Lights };
 	// without peer memory: this rank's light slot (the source fills it, a broadcast carries it to every rank) and, past
 	// its end, the flag words and counter of the source's push; allocated on the first such frame
 	void *light_slot = nullptr;
@@ -215,7 +243,6 @@ struct GrbhViewer
 	bool fed_from_source() const { return bands.size() > 1 && gbuffer_source >= 0; }
 	bool lights_from_source() const { return bands.size() > 1 && light_source >= 0; }
 	void exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count);
-	void raise_light_credit(Vulkan::CommandBuffer &cmd);
 
 	// the G-buffer planes of the attachments (grb_gbuffer_copy_rows order), the G-buffer ones and / or motion vectors
 	GrbGBufferPlanes attachment_planes(bool gbuffer_planes, bool mv)
@@ -347,7 +374,7 @@ void GrbhViewer::bake_render_graph()
 	if (lights_from_source())
 	{
 		device_lights.exchange = [this](Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count) { exchange_lights(cmd, list, count); };
-		device_lights.after_prep = [this](Vulkan::CommandBuffer &cmd) { raise_light_credit(cmd); };
+		device_lights.after_prep = [this](Vulkan::CommandBuffer &cmd) { light_handover.credit(cmd, rank); };
 	}
 	else
 	{
@@ -770,11 +797,9 @@ void GrbhViewer::set_output_ring(const GrbImage *images, int32_t count)
 		output_ring.emplace_back(new Vulkan::ImageView(std::make_shared<Vulkan::Image>(*device, info, images[i].data, (unsigned)images[i].row_pitch)));
 }
 
-// Feeding from the rank S that rasterised the whole frame (DESIGN.md section 5, "Feeding a sharded frame from one
-// rank").  Peer path: S waits for every rank's credit of the last epoch, pushes each rank q's input rows into q's slot
-// and copies its own; every other rank waits for S's flag, copies its rows out of its slot and raises its credit.
-// Without peer memory: S copies every rank's input rows into its own attachments, and per-plane NCCL broadcasts from
-// S write them into every rank's attachments in place.
+// Feeding from the rank S that rasterised the whole frame.  Peer path: S pushes each rank q's input rows into q's slot
+// and copies its own; every other rank copies its rows out of its slot.  Without peer memory: S copies every rank's
+// input rows into its own attachments, and per-plane NCCL broadcasts from S write them into every rank's in place.
 void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 {
 	const unsigned S = (unsigned)gbuffer_source;
@@ -794,13 +819,12 @@ void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 	if (!cmd.check(grb_gbuffer_slot_layout(&attachments, nullptr, nullptr, &bytes), "grb_gbuffer_slot_layout"))
 		return;
 	RenderGraphCollectives *coll = graph.get_collectives();
-	RenderGraphCollectives::PeerSlot slot;
-	if (coll->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::GBuffer, (size_t)bytes, slot))
+	if (gbuffer_handover.begin(cmd, *coll, (size_t)bytes, S, rank))
 	{
+		const RenderGraphCollectives::PeerSlot &slot = gbuffer_handover.slot;
+		const std::vector<GrbRows> own = upload_ranges();
 		if (rank == S)
 		{
-			// the credits: every rank copied the last epoch's rows out of its slot, and by stream order the epoch's before
-			cmd.check(grb_peer_wait(slot.flags[S], (int32_t)slot.count, slot.epoch - 1u, handle), "grb_peer_wait");
 			std::vector<GrbRows> rows;
 			std::vector<int32_t> counts;
 			for (unsigned q = 0; q < slot.count; q++)
@@ -812,21 +836,14 @@ void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 			cmd.check(grb_gbuffer_rows_to_peers(&src, slot.images, slot.flags, rows.data(), counts.data(), (int32_t)slot.count, (int32_t)S, slot.epoch,
 			                                    slot.counter, handle),
 			          "grb_gbuffer_rows_to_peers");
-			const std::vector<GrbRows> own = upload_ranges();
 			cmd.check(grb_gbuffer_copy_rows(&src, &attachments, own.data(), (int32_t)own.size(), handle), "grb_gbuffer_copy_rows");
 			record_consumed(stream, *in);
 			return;
 		}
-		cmd.check(grb_peer_wait(slot.flags[rank] + S, 1, slot.epoch, handle), "grb_peer_wait");
 		GrbGBufferPlanes received = {};
 		cmd.check(grb_gbuffer_slot_layout(&attachments, slot.images[rank], &received, &bytes), "grb_gbuffer_slot_layout");
-		const std::vector<GrbRows> own = upload_ranges();
 		cmd.check(grb_gbuffer_copy_rows(&received, &attachments, own.data(), (int32_t)own.size(), handle), "grb_gbuffer_copy_rows");
-		// the credit: a flags-only publish once the rows are out of the slot
-		const std::vector<int32_t> none(slot.count, 0);
-		cmd.check(grb_gbuffer_rows_to_peers(&attachments, nullptr, slot.flags, nullptr, none.data(), (int32_t)slot.count, (int32_t)rank, slot.epoch,
-		                                    slot.counter, handle),
-		          "grb_gbuffer_rows_to_peers");
+		gbuffer_handover.credit(cmd, rank);
 		return;
 	}
 	// without peer memory: the union of every rank's input rows, broadcast from S
@@ -860,11 +877,11 @@ void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 }
 
 // The light channel of a row-sharded frame whose device lights come from rank S (DESIGN.md section 5, "Lights from
-// device memory", "From one rank"), on the clustering pass's stream after the lights' `ready`.  Peer path: S waits for
-// every rank's credit of the last epoch and pushes its list's live entries into every rank's slot, then preps its own
-// list; every other rank waits for S's flag, preps its slot (the list and count returned here) and raises its credit
-// behind the prep (raise_light_credit).  Without peer memory: S fills its own slot with the same kernel and a broadcast
-// from S carries the whole slot into every rank's, in stream order with the prep that reads it.
+// device memory", "From one rank"), on the clustering pass's stream after the lights' `ready`.  Peer path: S pushes its
+// list's live entries into every rank's slot, then preps its own list; every other rank preps its slot (the list and
+// count returned here) and raises its credit behind the prep (`after_prep`).  Without peer memory: S fills its own
+// slot with the same kernel and a broadcast from S carries the whole slot into every rank's, in stream order with the
+// prep that reads it.
 void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count)
 {
 	const unsigned S = (unsigned)light_source;
@@ -873,21 +890,16 @@ void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list,
 	if (!cmd.check(grb_light_slot_layout(nullptr, nullptr, nullptr, &bytes), "grb_light_slot_layout"))
 		return;
 	RenderGraphCollectives *coll = graph.get_collectives();
-	RenderGraphCollectives::PeerSlot slot;
 	void *received = nullptr;
-	if (coll->peer_exchange_begin_frame(RenderGraphCollectives::PeerChannel::Lights, (size_t)bytes, slot))
+	if (light_handover.begin(cmd, *coll, (size_t)bytes, S, rank))
 	{
+		const RenderGraphCollectives::PeerSlot &slot = light_handover.slot;
 		if (rank == S)
 		{
-			// the credits: every rank's prep of the last epoch has read its slot, and by stream order the epoch's before
-			cmd.check(grb_peer_wait(slot.flags[S], (int32_t)slot.count, slot.epoch - 1u, handle), "grb_peer_wait");
 			cmd.check(grb_light_list_to_peers(&list, count, slot.images, slot.flags, (int32_t)slot.count, (int32_t)S, slot.epoch, slot.counter, handle),
 			          "grb_light_list_to_peers");
 			return;
 		}
-		cmd.check(grb_peer_wait(slot.flags[rank] + S, 1, slot.epoch, handle), "grb_peer_wait");
-		light_credit = slot;
-		light_credit_pending = true;
 		received = slot.images[rank];
 	}
 	else
@@ -925,17 +937,6 @@ void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list,
 	slot_list.cutoff_range = list.cutoff_range;
 	list = slot_list;
 	count = slot_count;
-}
-
-// A receiving rank's credit of the light channel: a flags-only publish behind the prep, the last read of its slot
-void GrbhViewer::raise_light_credit(Vulkan::CommandBuffer &cmd)
-{
-	if (!light_credit_pending)
-		return;
-	light_credit_pending = false;
-	cmd.check(grb_light_list_to_peers(nullptr, nullptr, nullptr, light_credit.flags, (int32_t)light_credit.count, (int32_t)rank, light_credit.epoch,
-	                                  light_credit.counter, cmd.get_stream_handle()),
-	          "grb_light_list_to_peers");
 }
 
 cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)

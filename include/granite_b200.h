@@ -251,12 +251,11 @@ int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t **count_out
  * slot's count word.  No entry at or past live is read.  16-byte loads and stores where the array and every slot are
  * 16-byte aligned, 4-byte ones for the float arrays where they are 4-byte aligned, bytes otherwise.  Then flags[flag_index] =
  * epoch is release-stored into the flag array of EVERY rank.  The grid is sized from the capacity (lights->count):
- * the length is not known on the host.  peer_slots may be NULL: a flags-only publish (the credit a receiving rank
- * raises once its prep has read its slot), for which lights and input_count may be NULL.  scratch_counter: one
- * zero-initialised uint32 in local device memory.  GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside
- * 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, a count outside 0..GRB_MAX_LIGHT_LIST, an input count that is not
- * 4-byte aligned, a slot that is not 16-byte aligned (checked before any CUDA call; nothing is written).  No reference
- * equivalent (the reference never splits a frame). */
+ * the length is not known on the host.  A receiver's credit, once its prep has read its slot, is grb_peer_publish.
+ * scratch_counter: one zero-initialised uint32 in local device memory.  GRB_ERR_INVALID_ARGUMENT: a null pointer,
+ * peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, a count outside 0..GRB_MAX_LIGHT_LIST, an
+ * input count that is not 4-byte aligned, a slot that is not 16-byte aligned (checked before any CUDA call; nothing is
+ * written).  No reference equivalent (the reference never splits a frame). */
 int32_t grb_light_list_to_peers(const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
                                 int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream);
 
@@ -432,6 +431,10 @@ int32_t grb_bloom_threshold_downsample_to_peers(const GrbImage *hdr, const float
                                                 void *stream);
 /* Stream-ordered wait until local_flags[0..count) have all reached `epoch` (acquire, system scope). */
 int32_t grb_peer_wait(const uint32_t *local_flags, int32_t count, uint32_t epoch, void *stream);
+/* A flags-only publish, the credit of a rank that receives a channel one source rank fills (grb_gbuffer_rows_to_peers,
+ * grb_light_list_to_peers), behind its last read of its slot: one CTA release-stores `epoch` into word flag_index of
+ * the flag array of EVERY rank and resets scratch_counter.  GRB_ERR_INVALID_ARGUMENT as grb_bloom_downsample_to_peers. */
+int32_t grb_peer_publish(uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream);
 /* K9 bloom_upsample.comp; hdr.cpp:189-216. */
 int32_t grb_bloom_upsample(const GrbImage *in, const GrbImage *out, GrbRows rows, void *stream);
 /* Same, never through the tile kernel: the shader's arithmetic statement for statement at every size (bit-exact to the
@@ -606,11 +609,11 @@ int32_t grb_gbuffer_slot_layout(const GrbGBufferPlanes *layout, void *base, GrbG
  * the lists of rows one after another, empty ranges allowed) of every present plane of src into peer_slots[q], the
  * base address, valid on this device, of rank q's slot (cudaIpc-mapped peer memory; the layout of
  * grb_gbuffer_slot_layout for src's planes), rows at their place.  Then flags[flag_index] = epoch is release-stored
- * into the flag array of EVERY rank.  peer_slots may be NULL when no range is listed: a flags-only publish (the credit a
- * receiving rank raises once it has copied its rows out of its slot).  scratch_counter: one zero-initialised uint32 in
- * local device memory.  GRB_ERR_INVALID_ARGUMENT: a null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index
- * outside 0..peer_count-1, a negative count, src's planes as for grb_gbuffer_copy_rows, a range outside the image
- * (checked before any CUDA call; nothing is written).  No reference equivalent (the reference never splits a frame). */
+ * into the flag array of EVERY rank.  A receiver's credit, once it has copied its rows out of its slot, is
+ * grb_peer_publish.  scratch_counter: one zero-initialised uint32 in local device memory.  GRB_ERR_INVALID_ARGUMENT: a
+ * null pointer, peer_count outside 1..GRB_MAX_PEERS, flag_index outside 0..peer_count-1, a negative count, src's
+ * planes as for grb_gbuffer_copy_rows, a range outside the image (checked before any CUDA call; nothing is written).
+ * No reference equivalent (the reference never splits a frame). */
 int32_t grb_gbuffer_rows_to_peers(const GrbGBufferPlanes *src, void *const *peer_slots, uint32_t *const *peer_flags, const GrbRows *rows,
                                   const int32_t *range_counts, int32_t peer_count, int32_t flag_index, uint32_t epoch,
                                   uint32_t *scratch_counter, void *stream);

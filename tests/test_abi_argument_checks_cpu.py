@@ -177,6 +177,24 @@ def test_bloom_to_peers_argument_checks(lib):
     assert all(a.sum() == 0 for a in keep[2:])
 
 
+def test_peer_publish_argument_checks(lib):
+    """grb_peer_publish (the flags-only publish of a receiving rank's credit) refuses null flag arrays, a null flag array
+    among them, a null counter, a peer_count of 0 or GRB_MAX_PEERS + 1 (9) and a flag_index of -1 or peer_count, each
+    before any CUDA call, with its message, and writes nothing."""
+    keep = [np.zeros(16, np.uint32) for _ in range(9)]
+    flags = (C.c_void_p * 9)(*[a.ctypes.data for a in keep])
+    counter = C.c_void_p(keep[0].ctypes.data + 32)
+
+    def call(fl=flags, n=2, k=0, ctr=counter):
+        return lib.grb_peer_publish(fl, n, k, C.c_uint32(1), ctr, None)
+
+    peers = "grb_peer_publish: null pointer, peer_count outside 1..GRB_MAX_PEERS or flag_index outside 0..peer_count-1"
+    for bad in (dict(fl=None), dict(ctr=None), dict(n=0), dict(n=9), dict(k=-1), dict(k=2), dict(n=8, k=8)):
+        assert call(**bad) == ERR_ARG and peers in _msg(lib), bad
+    assert call(fl=(C.c_void_p * 2)(keep[0].ctypes.data, None)) == ERR_ARG and "grb_peer_publish: null peer flag array" in _msg(lib)
+    assert not any(a.any() for a in keep), "a refused call wrote something"
+
+
 def test_lighting_rejects_misaligned_lights(lib):
     """Every lighting form reads the light records as float4, so a light table that is not 16-byte aligned is refused
     before any CUDA call, by the lighting pass and by its row-cost estimate."""

@@ -139,16 +139,16 @@ def test_rows_to_peers_argument_checks(viewer):
     assert call(fl=None) == ERR_ARG
     assert call(ctr=None) == ERR_ARG
     assert call(fl=(C.c_void_p * 2)(keep[2].ctypes.data, None)) == ERR_ARG and "null peer" in _msg(L)
-    assert call(sl=None, r=None, counts=(0, 0), fl=(C.c_void_p * 2)(keep[2].ctypes.data, None)) == ERR_ARG and "null peer flag" in _msg(L)
     assert call(sl=(C.c_void_p * 2)(keep[0].ctypes.data, None)) == ERR_ARG and "null peer pointer" in _msg(L)
     assert call(n=0) == ERR_ARG and "peer_count" in _msg(L)
     assert call(n=9, counts=(0,) * 9) == ERR_ARG
     assert call(k=2) == ERR_ARG and "flag_index" in _msg(L)
     assert call(k=-1) == ERR_ARG
     assert call(counts=(2, -1)) == ERR_ARG and "negative" in _msg(L)
-    # rows without slots (only a flags-only publish may leave them out), or without a list
-    assert call(sl=None) == ERR_ARG and "flags-only" in _msg(L)
-    assert call(r=None) == ERR_ARG
+    # no slots, also with no rows listed (the credit is grb_peer_publish); rows listed without a list
+    assert call(sl=None) == ERR_ARG and "grb_gbuffer_rows_to_peers: null pointer" in _msg(L)
+    assert call(sl=None, r=None, counts=(0, 0)) == ERR_ARG and "grb_gbuffer_rows_to_peers: null pointer" in _msg(L)
+    assert call(r=None) == ERR_ARG and "row list" in _msg(L)
     # a bad plane, a range outside the image
     bad = capi.GrbGBufferPlanes.from_buffer_copy(src)
     bad.plane[3].row_pitch = w * 2 - 2

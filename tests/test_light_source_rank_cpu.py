@@ -121,7 +121,7 @@ def _peer_args(n=2):
 
 def test_list_to_peers_refuses_before_any_cuda_call(built):
     """grb_light_list_to_peers refuses, with GRB_ERR_INVALID_ARGUMENT and its message: a null pointer (flag arrays,
-    counter, light list, array), peer_count outside 1..8, a flag_index outside 0..peer_count-1, a count outside
+    counter, slots, light list, array), peer_count outside 1..8, a flag_index outside 0..peer_count-1, a count outside
     0..65536, a misaligned count and a misaligned slot."""
     from granite_b200 import capi
 
@@ -137,7 +137,8 @@ def test_list_to_peers_refuses_before_any_cuda_call(built):
                  (C.byref(ll), None, slots, flags, 9, 0, 1, d, None),
                  (C.byref(ll), None, slots, flags, 2, -1, 1, d, None),
                  (C.byref(ll), None, slots, flags, 2, 2, 1, d, None),
-                 (None, None, None, flags, 2, 2, 1, d, None)):  # a flags-only publish is checked the same way
+                 (C.byref(ll), None, None, flags, 2, 0, 1, d, None),  # null slots (the credit is grb_peer_publish)
+                 (None, None, None, flags, 2, 2, 1, d, None)):
         assert fn(*args) == -1
         assert peers in L.grb_last_error_string()
     nulls = (C.c_void_p * 2)(4096, None)

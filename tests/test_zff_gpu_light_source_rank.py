@@ -1,7 +1,7 @@
 """Device lights pushed from one rank, on one GPU: grb_light_list_to_peers pushes a capacity-8192 list into three slot
 tensors of one device (the slots every rank of a row-sharded frame would hold), with counts from 0 to the capacity and
 the clamps; the slots, the count words, the flags and the scratch counter are checked, and the counted prep of every
-slot must equal the prep of the source list bit for bit.  Also the flags-only publish, and the refusal that needs a
+slot must equal the prep of the source list bit for bit.  Also a receiver's credit, and the refusal that needs a
 baked viewer."""
 import ctypes as C
 
@@ -99,8 +99,8 @@ def test_push_into_three_slots_and_prep_parity(cuda, oracle):
 
 
 def test_no_count_pushes_the_whole_list_and_flags_only_publish_stores_nothing(cuda):
-    """Without a device count every entry is live; a flags-only publish (no slots, no list) raises the flags at its
-    epoch and stores nothing."""
+    """Without a device count every entry is live; a receiver's credit, the flags-only publish of grb_peer_publish,
+    raises the flags at its epoch and stores nothing."""
     import torch
 
     from granite_b200 import harness, synth
@@ -118,7 +118,7 @@ def test_no_count_pushes_the_whole_list_and_flags_only_publish_stores_nothing(cu
         assert int(s[:4].view(torch.int32).item()) == 37
         assert torch.equal(s[256 + 16 * 0:256 + 37 * 12], d["color"].reshape(-1).view(torch.uint8))
     before = [s.clone() for s in slots]
-    harness.light_list_to_peers(None, None, None, flags, 0, 8, counter)
+    harness.peer_publish(flags, 0, 8, counter)
     torch.cuda.synchronize()
     assert [f[:2].tolist() for f in flags] == [[8, 7], [8, 7]]
     assert int(counter.item()) == 0

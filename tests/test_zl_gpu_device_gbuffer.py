@@ -78,8 +78,8 @@ def test_copy_rows_writes_only_the_listed_rows(cuda, fp16, width, pitch_texels, 
 def test_rows_to_peers_routes_each_ranks_rows(cuda, width, pitch_texels):
     """Two allocations stand in for two ranks' G-buffer slots; rank 1 is the source.  Each rank's slot receives exactly
     its listed rows of every plane at their place in the slot layout, every other byte stays the sentinel; every flag
-    array gets the epoch at the caller's index; the scratch counter is reset.  Then a flags-only publish from rank 0
-    (the credit) raises its word and writes nothing."""
+    array gets the epoch at the caller's index; the scratch counter is reset.  Then rank 0's credit (grb_peer_publish)
+    raises its word and writes nothing."""
     import torch
 
     from granite_b200 import capi, harness
@@ -108,7 +108,7 @@ def test_rows_to_peers_routes_each_ranks_rows(cuda, width, pitch_texels):
         assert list(f.cpu().numpy()) == [0, 5] + [0] * 14
     assert counter.item() == 0
     before = [s.clone() for s in slots]
-    harness.gbuffer_rows_to_peers(src, None, flags, [[], []], 0, 6, counter)
+    harness.peer_publish(flags, 0, 6, counter)
     torch.cuda.synchronize()
     for f in flags:
         assert list(f.cpu().numpy()) == [6, 5] + [0] * 14
