@@ -107,6 +107,12 @@ class GrbLightList(C.Structure):
 MAX_LIGHT_LIST = 65536  # GRB_MAX_LIGHT_LIST
 
 
+class GrbLightShadowIdList(C.Structure):
+    """The shadows of a GrbLightList by map id (grb_light_prep_shadow_ids / grb_light_list_shadowed_to_peers): device
+    arrays of count x 16 float32 transforms and count int32 map ids."""
+    _fields_ = [("transforms", C.c_void_p), ("map_ids", C.c_void_p)]
+
+
 class GrbLightShadows(C.Structure):
     _fields_ = [("transforms", C.c_void_p), ("maps", C.c_void_p), ("resolution", C.c_int32), ("pcf_wide", C.c_int32)]
 
@@ -122,6 +128,7 @@ ENTRY_POINTS = [
     "grb_pq10_encode", "grb_smaa_edge_detection", "grb_smaa_edge_detection_to_peers", "grb_smaa_blend_weights", "grb_smaa_neighborhood_blend", "grb_fsr_easu_constants", "grb_fsr_upscale", "grb_fsr_sharpen", "grb_fxaa", "grb_taa_resolve", "grb_taa_resolve_to_peers",
     "grb_present_rows_to_peer", "grb_deferred_lighting_stripes", "grb_hdr_rows_to_peers",
     "grb_gbuffer_copy_rows", "grb_gbuffer_slot_layout", "grb_gbuffer_rows_to_peers", "grb_light_slot_layout", "grb_light_list_to_peers",
+    "grb_light_prep_shadow_ids", "grb_light_shadow_slot_layout", "grb_light_list_shadowed_to_peers",
 ]
 
 _lib = None
@@ -187,6 +194,9 @@ def lib() -> C.CDLL:
             "grb_gbuffer_rows_to_peers": [C.POINTER(GrbGBufferPlanes), P, P, C.POINTER(GrbRows), C.POINTER(C.c_int32), I, I, C.c_uint32, P, P],
             "grb_light_slot_layout": [P, C.POINTER(GrbLightList), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)],
             "grb_light_list_to_peers": [C.POINTER(GrbLightList), P, P, P, I, I, C.c_uint32, P, P],
+            "grb_light_prep_shadow_ids": [C.POINTER(GrbLightList), P, C.POINTER(GrbLightShadowIdList), P, I, P, P, P, P, P, P, P, P, P, C.c_uint64, P],
+            "grb_light_shadow_slot_layout": [P, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)],
+            "grb_light_list_shadowed_to_peers": [C.POINTER(GrbLightList), C.POINTER(GrbLightShadowIdList), P, P, P, I, I, C.c_uint32, P, P],
         }
         for name, args in sig.items():
             fn = getattr(_lib, name)

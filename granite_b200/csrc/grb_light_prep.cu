@@ -10,12 +10,14 @@
 //      by_key_then_input comparator;
 //   3. pack_kernel, one thread per slot of GRB_MAX_CLUSTER_LIGHTS: the visible count is where the culled keys begin
 //      (a binary search of the sorted keys), and slot s < count packs sorted light s (grb_light_prep_shadowed: with its
-//      shadow transform and map).
+//      shadow transform and map; grb_light_prep_shadow_ids: with its transform and this rank's map of its map id).
 // The _counted forms read the list's live length on the device: step 1 gives every entry past it the culled key without
 // loading it, so steps 2 and 3 are unchanged and never reach those entries.
 //
 // grb_light_list_to_peers pushes a list's live entries from one rank into every rank's light slot (the protocol is
 // grb_peer.cuh's); each receiver then runs the counted prep on its slot, so every rank preps the same bytes.
+// grb_light_list_shadowed_to_peers pushes the shadow transforms and map ids with them, and each receiver resolves the ids
+// through its own map table (grb_light_prep_shadow_ids): a map pointer is valid on its own rank only, an id anywhere.
 #include "grb_common.cuh"
 #include "grb_light_prep.cuh"
 #include "grb_peer.cuh"
@@ -23,6 +25,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include <string>
+#include <type_traits>
 
 namespace grb
 {
@@ -44,9 +47,10 @@ __global__ void __launch_bounds__(256) cull_key_kernel(GrbLightList lights, cons
 	values[i] = (uint32_t)i;
 }
 
-// Shadowed: the shadow tables too (lp::pack_shadow); grb_light_prep runs the <false> form, whose code has no shadow part.
-template <bool Shadowed>
-__global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights, GrbLightShadowList shadows, GrbLightPrepView view,
+// Shadows: where the shadow tables come from (lp::pack_shadow) -- GrbLightShadowList by map pointer, lp::ShadowIds by map
+// id through a table; grb_light_prep runs the lp::NoShadows form, whose code has no shadow part.
+template <class Shadows>
+__global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights, Shadows shadows, GrbLightPrepView view,
                                                            const unsigned long long *__restrict__ keys, const uint32_t *__restrict__ order,
                                                            GrbPositionalLight *__restrict__ records, float *__restrict__ model,
                                                            uint32_t *__restrict__ type_mask, uint2 *__restrict__ z_ranges, float *__restrict__ shadow_transforms,
@@ -72,8 +76,9 @@ __global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights,
 	const int slots = min(lights.count, GRB_MAX_CLUSTER_LIGHTS);
 	const int s = blockIdx.x * blockDim.x + threadIdx.x;
 	bool point = false;
-	if (Shadowed && s < slots)
-		lp::pack_shadow(shadows, s < count ? (int)order[s] : -1, s, shadow_transforms, shadow_maps);
+	if constexpr (!std::is_same<Shadows, lp::NoShadows>::value)
+		if (s < slots)
+			lp::pack_shadow(shadows, s < count ? (int)order[s] : -1, s, shadow_transforms, shadow_maps);
 	if (s < count)
 	{
 		const lp::Light L = lp::load_light(lights, (int)order[s]);
@@ -105,8 +110,11 @@ __global__ void __launch_bounds__(kPackThreads) pack_kernel(GrbLightList lights,
 		*count_out = count;
 }
 
-// One thread per 16-byte chunk of the capacity's six arrays (lp::push_light_chunk), then the count word and the publish.
-__global__ void __launch_bounds__(256) light_push_kernel(lp::LightPush push, const int32_t *__restrict__ input_count, int capacity, PeerTargets targets)
+// One thread per 16-byte chunk of the capacity's arrays (lp::push_light_chunk: the six of the list, eight with the shadow
+// transforms and map ids), then the count word and the publish.
+template <int Arrays>
+__global__ void __launch_bounds__(256) light_push_kernel(lp::LightPushArrays<Arrays> push, const int32_t *__restrict__ input_count, int capacity,
+                                                         PeerTargets targets)
 {
 	const int live = input_count ? lp::live_count(*input_count, capacity) : capacity;
 	const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -159,9 +167,9 @@ extern "C" uint64_t grb_light_prep_scratch_bytes(int32_t max_lights)
 
 namespace
 {
-// grb_light_prep[_shadowed][_counted]: the checks of grb_light_prep, then the three steps; shadows null = the
-// unshadowed pack kernel, input_count null = every entry of the list is a light
-int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowList *shadows,
+// grb_light_prep[_shadowed][_counted] and grb_light_prep_shadow_ids: the checks of grb_light_prep, then the three steps;
+// shadows and ids null = the unshadowed pack kernel, input_count null = every entry of the list is a light
+int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowList *shadows, const lp::ShadowIds *ids,
                    const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges,
                    float *shadow_transforms, const void **shadow_maps, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
 {
@@ -180,6 +188,21 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *in
 	if (shadows && (((uintptr_t)shadow_transforms & 7) || ((uintptr_t)shadows->maps & 7) || ((uintptr_t)shadow_maps & 7)))
 	{
 		set_last_error((std::string(fn) + ": the output transforms, the map array or the output maps are not 8-byte aligned").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (ids && (!shadow_transforms || !shadow_maps || (lights->count > 0 && (!ids->ids.transforms || !ids->ids.map_ids))))
+	{
+		set_last_error((std::string(fn) + ": a null shadow transform or map id array, or a null output table").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (ids && (ids->table_size < 0 || ids->table_size > GRB_MAX_LIGHT_LIST || (ids->table_size > 0 && !ids->table)))
+	{
+		set_last_error((std::string(fn) + ": a map table size outside 0..GRB_MAX_LIGHT_LIST or a null map table").c_str());
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	if (ids && (((uintptr_t)shadow_transforms & 7) || ((uintptr_t)ids->table & 7) || ((uintptr_t)shadow_maps & 7) || ((uintptr_t)ids->ids.map_ids & 3)))
+	{
+		set_last_error((std::string(fn) + ": the output transforms, the map table or the output maps are not 8-byte aligned, or the map ids not 4-byte aligned").c_str());
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
 	if ((uintptr_t)input_count & 3)
@@ -214,12 +237,16 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *in
 			return check_launch((std::string(fn) + ": sort").c_str());
 	}
 	auto *ranges = reinterpret_cast<uint2 *>(z_ranges);
-	if (shadows)
-		pack_kernel<true><<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, *shadows, *view, keys_out, values_out, records, model,
-		                                                                                type_mask, ranges, shadow_transforms, shadow_maps, device_count);
+	constexpr int blocks = GRB_MAX_CLUSTER_LIGHTS / kPackThreads;
+	if (ids)
+		pack_kernel<lp::ShadowIds><<<blocks, kPackThreads, 0, s>>>(*lights, *ids, *view, keys_out, values_out, records, model, type_mask, ranges,
+		                                                           shadow_transforms, shadow_maps, device_count);
+	else if (shadows)
+		pack_kernel<GrbLightShadowList><<<blocks, kPackThreads, 0, s>>>(*lights, *shadows, *view, keys_out, values_out, records, model, type_mask, ranges,
+		                                                                shadow_transforms, shadow_maps, device_count);
 	else
-		pack_kernel<false><<<GRB_MAX_CLUSTER_LIGHTS / kPackThreads, kPackThreads, 0, s>>>(*lights, GrbLightShadowList{}, *view, keys_out, values_out, records,
-		                                                                                 model, type_mask, ranges, nullptr, nullptr, device_count);
+		pack_kernel<lp::NoShadows><<<blocks, kPackThreads, 0, s>>>(*lights, lp::NoShadows{}, *view, keys_out, values_out, records, model, type_mask, ranges,
+		                                                           nullptr, nullptr, device_count);
 	return check_launch((std::string(fn) + ": pack").c_str());
 }
 } // namespace
@@ -227,7 +254,7 @@ int32_t light_prep(const char *fn, const GrbLightList *lights, const int32_t *in
 extern "C" int32_t grb_light_prep(const GrbLightList *lights, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
                                   uint32_t *z_ranges, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
 {
-	return light_prep("grb_light_prep", lights, nullptr, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count, scratch,
+	return light_prep("grb_light_prep", lights, nullptr, nullptr, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count, scratch,
 	                  scratch_bytes, stream);
 }
 
@@ -240,7 +267,7 @@ extern "C" int32_t grb_light_prep_shadowed(const GrbLightList *lights, const Grb
 		set_last_error("grb_light_prep_shadowed: a null shadow table");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	return light_prep("grb_light_prep_shadowed", lights, nullptr, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out,
+	return light_prep("grb_light_prep_shadowed", lights, nullptr, shadows, nullptr, view, records, model, type_mask, z_ranges, shadow_transforms_out,
 	                  shadow_maps_out, device_count, scratch, scratch_bytes, stream);
 }
 
@@ -253,7 +280,7 @@ extern "C" int32_t grb_light_prep_counted(const GrbLightList *lights, const int3
 		set_last_error("grb_light_prep_counted: a null input count");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	return light_prep("grb_light_prep_counted", lights, input_count, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count,
+	return light_prep("grb_light_prep_counted", lights, input_count, nullptr, nullptr, view, records, model, type_mask, z_ranges, nullptr, nullptr, device_count,
 	                  scratch, scratch_bytes, stream);
 }
 
@@ -267,8 +294,23 @@ extern "C" int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, c
 		set_last_error("grb_light_prep_shadowed_counted: a null input count or shadow table");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	return light_prep("grb_light_prep_shadowed_counted", lights, input_count, shadows, view, records, model, type_mask, z_ranges, shadow_transforms_out,
+	return light_prep("grb_light_prep_shadowed_counted", lights, input_count, shadows, nullptr, view, records, model, type_mask, z_ranges, shadow_transforms_out,
 	                  shadow_maps_out, device_count, scratch, scratch_bytes, stream);
+}
+
+extern "C" int32_t grb_light_prep_shadow_ids(const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowIdList *ids,
+                                             const void *const *map_table, int32_t table_size, const GrbLightPrepView *view, GrbPositionalLight *records,
+                                             float *model, uint32_t *type_mask, uint32_t *z_ranges, float *shadow_transforms_out,
+                                             const void **shadow_maps_out, int32_t *device_count, void *scratch, uint64_t scratch_bytes, void *stream)
+{
+	if (!ids)
+	{
+		set_last_error("grb_light_prep_shadow_ids: a null shadow id list");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	const lp::ShadowIds shadow_ids{ *ids, map_table, table_size };
+	return light_prep("grb_light_prep_shadow_ids", lights, input_count, nullptr, &shadow_ids, view, records, model, type_mask, z_ranges,
+	                  shadow_transforms_out, shadow_maps_out, device_count, scratch, scratch_bytes, stream);
 }
 
 extern "C" int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t **count_out, uint64_t *bytes)
@@ -303,32 +345,87 @@ extern "C" int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t 
 	return GRB_OK;
 }
 
+namespace
+{
+// The checks of grb_light_list[_shadowed]_to_peers that need no CUDA call
+bool push_arguments(const char *fn, const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
+                    int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, PeerTargets &targets)
+{
+	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
+		return false;
+	if (!lights || lights->count < 0 || lights->count > GRB_MAX_LIGHT_LIST ||
+	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone || !lights->outer_cone)))
+	{
+		set_last_error((std::string(fn) + ": a null light list or array, or a count outside 0..GRB_MAX_LIGHT_LIST").c_str());
+		return false;
+	}
+	if ((uintptr_t)input_count & 3)
+	{
+		set_last_error((std::string(fn) + ": the input count is not 4-byte aligned").c_str());
+		return false;
+	}
+	for (int r = 0; r < peer_count; r++)
+		if ((uintptr_t)peer_slots[r] & 15)
+		{
+			set_last_error((std::string(fn) + ": a slot is not 16-byte aligned").c_str());
+			return false;
+		}
+	return true;
+}
+
+template <int Arrays>
+int32_t launch_push(const char *fn, const lp::LightPushArrays<Arrays> &push, const int32_t *input_count, int capacity, const PeerTargets &targets,
+                    void *stream)
+{
+	const unsigned blocks = (unsigned)((push.start[Arrays] + 255) / 256);
+	light_push_kernel<Arrays><<<blocks > 0 ? blocks : 1, 256, 0, as_stream(stream)>>>(push, input_count, capacity, targets);
+	return check_launch(fn);
+}
+} // namespace
+
 extern "C" int32_t grb_light_list_to_peers(const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
                                            int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream)
 {
 	const char *fn = "grb_light_list_to_peers";
 	PeerTargets targets;
-	if (!peer_targets_from(fn, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
+	if (!push_arguments(fn, lights, input_count, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
 		return GRB_ERR_INVALID_ARGUMENT;
-	if (!lights || lights->count < 0 || lights->count > GRB_MAX_LIGHT_LIST ||
-	    (lights->count > 0 && (!lights->color || !lights->position || !lights->is_point || !lights->rotation || !lights->inner_cone || !lights->outer_cone)))
+	return launch_push(fn, lp::light_push(*lights), input_count, lights->count, targets, stream);
+}
+
+extern "C" int32_t grb_light_shadow_slot_layout(void *slot, float **transforms, int32_t **map_ids, uint64_t *bytes)
+{
+	if (!bytes)
 	{
-		set_last_error("grb_light_list_to_peers: a null light list or array, or a count outside 0..GRB_MAX_LIGHT_LIST");
+		set_last_error("grb_light_shadow_slot_layout: a null size pointer");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	if ((uintptr_t)input_count & 3)
+	if ((uintptr_t)slot & 15)
 	{
-		set_last_error("grb_light_list_to_peers: the input count is not 4-byte aligned");
+		set_last_error("grb_light_shadow_slot_layout: the slot is not 16-byte aligned");
 		return GRB_ERR_INVALID_ARGUMENT;
 	}
-	for (int r = 0; r < peer_count; r++)
-		if ((uintptr_t)peer_slots[r] & 15)
-		{
-			set_last_error("grb_light_list_to_peers: a slot is not 16-byte aligned");
-			return GRB_ERR_INVALID_ARGUMENT;
-		}
-	const lp::LightPush push = lp::light_push(*lights);
-	const unsigned blocks = (unsigned)((push.start[lp::kLightArrays] + 255) / 256);
-	light_push_kernel<<<blocks > 0 ? blocks : 1, 256, 0, as_stream(stream)>>>(push, input_count, lights->count, targets);
-	return check_launch(fn);
+	*bytes = lp::shadow_array_offset(lp::kShadowedLightArrays);
+	auto *base = static_cast<uint8_t *>(slot);
+	if (transforms)
+		*transforms = base ? reinterpret_cast<float *>(base + lp::shadow_array_offset(lp::kLightArrays)) : nullptr;
+	if (map_ids)
+		*map_ids = base ? reinterpret_cast<int32_t *>(base + lp::shadow_array_offset(lp::kLightArrays + 1)) : nullptr;
+	return GRB_OK;
+}
+
+extern "C" int32_t grb_light_list_shadowed_to_peers(const GrbLightList *lights, const GrbLightShadowIdList *ids, const int32_t *input_count,
+                                                    void *const *peer_slots, uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index,
+                                                    uint32_t epoch, uint32_t *scratch_counter, void *stream)
+{
+	const char *fn = "grb_light_list_shadowed_to_peers";
+	PeerTargets targets;
+	if (!push_arguments(fn, lights, input_count, peer_slots, peer_flags, peer_count, flag_index, epoch, scratch_counter, targets))
+		return GRB_ERR_INVALID_ARGUMENT;
+	if (!ids || (lights->count > 0 && (!ids->transforms || !ids->map_ids)))
+	{
+		set_last_error("grb_light_list_shadowed_to_peers: a null shadow id list, or null transforms or map ids");
+		return GRB_ERR_INVALID_ARGUMENT;
+	}
+	return launch_push(fn, lp::light_shadow_push(*lights, *ids), input_count, lights->count, targets, stream);
 }

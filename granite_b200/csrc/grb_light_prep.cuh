@@ -218,48 +218,89 @@ __host__ __device__ inline LightSlotLayout light_slot_layout()
 	return l;
 }
 
-// What the push kernel of grb_light_list_to_peers copies: the six source arrays, laid end to end in 16-byte chunks of
-// which array a owns [start[a], start[a + 1]) (start[kLightArrays] = every chunk of the capacity), and whether array
-// a moves in 16-byte words (vec16) or 4-byte words (vec4) -- both sides aligned -- or else byte by byte.
-struct LightPush
+// The shadowed light slot of grb_light_shadow_slot_layout: the light slot, then the shadow transforms and the map ids of
+// GRB_MAX_LIGHT_LIST entries (arrays kLightArrays and kLightArrays + 1 of a shadowed push), each from a multiple of 256
+// bytes.  The shadow part's element sizes and offsets are separate functions, so that the unshadowed push keeps its code.
+constexpr int kShadowedLightArrays = kLightArrays + 2;
+__host__ __device__ inline int shadow_element_bytes(int a) { return a == kLightArrays ? 64 : 4; }
+// the offset of array a >= kLightArrays of a shadowed slot (a == kShadowedLightArrays: the shadowed slot's size)
+__host__ __device__ inline uint64_t shadow_array_offset(int a)
 {
-	const uint8_t *src[kLightArrays];
-	int start[kLightArrays + 1];
+	uint64_t at = light_array_offset(kLightArrays);
+	for (int k = kLightArrays; k < a; k++)
+		at += ((uint64_t)GRB_MAX_LIGHT_LIST * (uint64_t)shadow_element_bytes(k) + 255) / 256 * 256;
+	return at;
+}
+// element size and slot offset of array a of a push of Arrays arrays (kLightArrays: the light slot's only)
+template <int Arrays>
+__host__ __device__ inline int push_element_bytes(int a)
+{
+	return Arrays == kLightArrays || a < kLightArrays ? light_element_bytes(a) : shadow_element_bytes(a);
+}
+template <int Arrays>
+__host__ __device__ inline uint64_t push_array_offset(int a)
+{
+	return Arrays == kLightArrays || a < kLightArrays ? light_array_offset(a) : shadow_array_offset(a);
+}
+
+// What the push kernel of grb_light_list[_shadowed]_to_peers copies: the Arrays source arrays (the six of the light
+// list, then for a shadowed list the transforms and the map ids), laid end to end in 16-byte chunks of which array a
+// owns [start[a], start[a + 1]) (start[Arrays] = every chunk of the capacity), and whether array a moves in 16-byte
+// words (vec16) or 4-byte words (vec4) -- both sides aligned -- or else byte by byte.
+template <int Arrays>
+struct LightPushArrays
+{
+	const uint8_t *src[Arrays];
+	int start[Arrays + 1];
 	unsigned vec16, vec4;
 };
+using LightPush = LightPushArrays<kLightArrays>;
+using LightShadowPush = LightPushArrays<kShadowedLightArrays>;
 
-// The push of `lights` (count = its capacity): each array's source and chunk range, and the word size both sides allow
+// The push of `src` (capacity entries each): each array's source and chunk range, and the word size both sides allow
 // (the slots are 16-byte aligned and every array of a slot starts on a multiple of 256 bytes).
-inline LightPush light_push(const GrbLightList &lights)
+template <int Arrays>
+inline LightPushArrays<Arrays> light_push_arrays(const void *const *src, int capacity)
 {
-	LightPush push = {};
-	const void *src[kLightArrays] = { lights.color, lights.position, lights.is_point, lights.rotation, lights.inner_cone, lights.outer_cone };
+	LightPushArrays<Arrays> push = {};
 	push.start[0] = 0;
-	for (int a = 0; a < kLightArrays; a++)
+	for (int a = 0; a < Arrays; a++)
 	{
 		push.src[a] = static_cast<const uint8_t *>(src[a]);
 		const uintptr_t p = reinterpret_cast<uintptr_t>(src[a]);
 		if ((p & 15) == 0)
 			push.vec16 |= 1u << a;
-		if (light_element_bytes(a) % 4 == 0 && (p & 3) == 0)
+		if (push_element_bytes<Arrays>(a) % 4 == 0 && (p & 3) == 0)
 			push.vec4 |= 1u << a;
-		push.start[a + 1] = push.start[a] + (lights.count * light_element_bytes(a) + 15) / 16;
+		push.start[a + 1] = push.start[a] + (capacity * push_element_bytes<Arrays>(a) + 15) / 16;
 	}
 	return push;
+}
+inline LightPush light_push(const GrbLightList &lights)
+{
+	const void *src[kLightArrays] = { lights.color, lights.position, lights.is_point, lights.rotation, lights.inner_cone, lights.outer_cone };
+	return light_push_arrays<kLightArrays>(src, lights.count);
+}
+inline LightShadowPush light_shadow_push(const GrbLightList &lights, const GrbLightShadowIdList &ids)
+{
+	const void *src[kShadowedLightArrays] = { lights.color,      lights.position,   lights.is_point,  lights.rotation,
+		                                      lights.inner_cone, lights.outer_cone, ids.transforms,   ids.map_ids };
+	return light_push_arrays<kShadowedLightArrays>(src, lights.count);
 }
 
 // Thread t of the push: chunk t's bytes that lie below live x element size of its array, loaded once and stored at the
 // same offset of that array in each of the `count` (<= GRB_MAX_PEERS) slots; nothing at or past it is read.  The loops
 // over the arrays and the slots unroll, so that the kernel indexes its parameters with constants only.
-__host__ __device__ inline void push_light_chunk(const LightPush &p, int live, int t, void *const *slots, int count)
+template <int Arrays>
+__host__ __device__ inline void push_light_chunk(const LightPushArrays<Arrays> &p, int live, int t, void *const *slots, int count)
 {
-	if (t >= p.start[kLightArrays])
+	if (t >= p.start[Arrays])
 		return;
 	int a = 0;
 	const uint8_t *src = p.src[0];
 	int first = 0;
 #pragma unroll
-	for (int k = 1; k < kLightArrays; k++)
+	for (int k = 1; k < Arrays; k++)
 		if (t >= p.start[k])
 		{
 			a = k;
@@ -267,11 +308,11 @@ __host__ __device__ inline void push_light_chunk(const LightPush &p, int live, i
 			first = p.start[k];
 		}
 	const uint64_t at = 16ull * (uint64_t)(t - first);
-	const uint64_t end = (uint64_t)live * (uint64_t)light_element_bytes(a);
+	const uint64_t end = (uint64_t)live * (uint64_t)push_element_bytes<Arrays>(a);
 	if (at >= end)
 		return;
 	const int n = end - at < 16 ? (int)(end - at) : 16;
-	const uint64_t dst = light_array_offset(a) + at;
+	const uint64_t dst = push_array_offset<Arrays>(a) + at;
 	const uint8_t *s = src + at;
 	if (n == 16 && ((p.vec16 >> a) & 1u))
 	{
@@ -283,7 +324,7 @@ __host__ __device__ inline void push_light_chunk(const LightPush &p, int live, i
 	}
 	else if ((p.vec4 >> a) & 1u)
 	{
-		// n is a multiple of 4 here: the arrays that move in 4-byte words have 4-byte elements
+		// n is a multiple of 4 here: the arrays that move in 4-byte words have elements of a multiple of 4 bytes
 		for (int j = 0; j < n; j += 4)
 		{
 			const uint32_t v = *reinterpret_cast<const uint32_t *>(s + j);
@@ -407,18 +448,42 @@ __host__ __device__ inline void pack(const Light &L, const GrbLightPrepView &vie
 	zr[1] = uy < (uint32_t)view.z_max_index ? uy : (uint32_t)view.z_max_index;
 }
 
+// Where the pack kernel's shadow part finds a light's map: by pointer (GrbLightShadowList, grb_light_prep_shadowed), or
+// by id through this rank's table (ShadowIds, grb_light_prep_shadow_ids).  The unshadowed pack has no shadow part; its
+// parameter keeps GrbLightShadowList's size, so that the kernel's parameter layout and code stay those of before.
+struct NoShadows
+{
+	const void *unused[2];
+};
+struct ShadowIds
+{
+	GrbLightShadowIdList ids;
+	const void *const *table;
+	int table_size;
+};
+__host__ __device__ inline const float *shadow_transforms(const GrbLightShadowList &s) { return s.transforms; }
+__host__ __device__ inline const float *shadow_transforms(const ShadowIds &s) { return s.ids.transforms; }
+__host__ __device__ inline const void *shadow_map(const GrbLightShadowList &s, int src) { return s.maps[src]; }
+// an id written on the device cannot be refused: one outside 0..table_size - 1 (negative ones included) means no shadow
+__host__ __device__ inline const void *shadow_map(const ShadowIds &s, int src)
+{
+	const int32_t id = s.ids.map_ids[src];
+	return (uint32_t)id < (uint32_t)s.table_size ? s.table[id] : nullptr;
+}
+
 // The shadow tables of slot s < slots: the transform and map of input light `src` (>= 0), or a zero matrix and a null
 // map (src < 0).  The input transform is read one float at a time (it may be only 4-byte aligned); the output starts at
 // packed_size(slots) of "cluster-transforms", 8-byte aligned for odd slot counts, so it is stored as float2.
-__host__ __device__ inline void pack_shadow(const GrbLightShadowList &shadows, int src, int s, float *transforms_out, const void **maps_out)
+template <class Shadows>
+__host__ __device__ inline void pack_shadow(const Shadows &shadows, int src, int s, float *transforms_out, const void **maps_out)
 {
 	float2 *t = reinterpret_cast<float2 *>(transforms_out + 16 * (size_t)s);
 	if (src >= 0)
 	{
-		const float *m = shadows.transforms + 16 * (size_t)src;
+		const float *m = shadow_transforms(shadows) + 16 * (size_t)src;
 		for (int k = 0; k < 8; k++)
 			t[k] = make_float2(m[2 * k], m[2 * k + 1]);
-		maps_out[s] = shadows.maps[src];
+		maps_out[s] = shadow_map(shadows, src);
 	}
 	else
 	{

@@ -443,6 +443,41 @@ def light_list_to_peers(lights, input_count_t, slots, flag_arrays, flag_index, e
                "grb_light_list_to_peers")
 
 
+def light_prep_shadow_ids(lights, input_count_t, transforms_t, map_ids_t, table_t, view, records_t, model_t, type_mask_t, z_ranges_t,
+                          shadow_transforms_t, shadow_maps_t, count_t, scratch_t):
+    """grb_light_prep_shadow_ids on the current stream: lights a GrbLightList, view a GrbLightPrepView, every other
+    argument a CUDA tensor (input_count_t None: every entry live); table_t an int64 tensor of map pointers whose length
+    is the table's size; the outputs as grb_light_prep_shadowed takes them."""
+    ids = capi.GrbLightShadowIdList(_ptr(transforms_t), _ptr(map_ids_t))
+    capi.check(capi.lib().grb_light_prep_shadow_ids(C.byref(lights), _ptr(input_count_t), C.byref(ids), _ptr(table_t), int(table_t.numel()), C.byref(view),
+                                                    _ptr(records_t), _ptr(model_t), _ptr(type_mask_t), _ptr(z_ranges_t), _ptr(shadow_transforms_t),
+                                                    _ptr(shadow_maps_t), _ptr(count_t), _ptr(scratch_t), scratch_t.numel() * scratch_t.element_size(),
+                                                    capi.stream_ptr()),
+               "grb_light_prep_shadow_ids")
+
+
+def light_shadow_slot_layout(base=None):
+    """grb_light_shadow_slot_layout: (the transforms' address, the map ids' address, the whole shadowed slot's bytes) of a
+    slot at device address `base`; base None queries the size (null addresses)."""
+    t, m, size = C.c_void_p(), C.c_void_p(), C.c_uint64()
+    capi.check(capi.lib().grb_light_shadow_slot_layout(None if base is None else C.c_void_p(base), C.byref(t), C.byref(m), C.byref(size)),
+               "grb_light_shadow_slot_layout")
+    return t.value, m.value, size.value
+
+
+def light_list_shadowed_to_peers(lights, transforms_t, map_ids_t, input_count_t, slots, flag_arrays, flag_index, epoch, counter_t):
+    """grb_light_list_shadowed_to_peers with every rank's slot and flag array as tensors on this device: lights a
+    GrbLightList, transforms_t / map_ids_t its shadow transforms and map ids, slots[r] a uint8 tensor of the shadowed
+    slot's bytes."""
+    n = len(flag_arrays)
+    ids = capi.GrbLightShadowIdList(_ptr(transforms_t), _ptr(map_ids_t))
+    images = (C.c_void_p * n)(*[t.data_ptr() for t in slots])
+    flags = (C.c_void_p * n)(*[t.data_ptr() for t in flag_arrays])
+    capi.check(capi.lib().grb_light_list_shadowed_to_peers(C.byref(lights), C.byref(ids), _ptr(input_count_t), images, flags, n, int(flag_index), int(epoch),
+                                                           _ptr(counter_t), capi.stream_ptr()),
+               "grb_light_list_shadowed_to_peers")
+
+
 def to_dev(a):
     return _dev(a)
 

@@ -453,15 +453,20 @@ void LightClusterer::build_cluster_bindless_gpu(Vulkan::CommandBuffer &cmd)
 		void *s = cmd.get_stream_handle();
 		GrbLightList list = src.list;
 		const int32_t *input_count = src.input_count;
+		GrbLightShadowIdList ids = src.shadow_ids;
 		if (src.exchange)
-			src.exchange(cmd, list, input_count);
+			src.exchange(cmd, list, input_count, ids);
 		if (enable_shadows)
 		{
 			// the shadow tables where the lighting pass reads them: packed_size(slots) and packed_offset_shadow_maps(slots)
 			const GrbLightShadows out = get_light_shadows();
 			auto *transforms = const_cast<float *>(out.transforms);
 			auto *maps = const_cast<const void **>(out.maps);
-			if (input_count)
+			if (src.by_id)
+				cmd.check(grb_light_prep_shadow_ids(&list, input_count, &ids, src.map_table, src.map_table_size, &device_view, records, model, type_mask,
+				                                    z_ranges, transforms, maps, src.count, src.scratch, src.scratch_bytes, s),
+				          "grb_light_prep_shadow_ids");
+			else if (input_count)
 				cmd.check(grb_light_prep_shadowed_counted(&list, input_count, &src.shadows, &device_view, records, model, type_mask, z_ranges,
 				                                          transforms, maps, src.count, src.scratch, src.scratch_bytes, s),
 				          "grb_light_prep_shadowed_counted");

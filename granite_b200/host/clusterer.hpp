@@ -100,15 +100,21 @@ public:
 	// `input_count` (device, or null = all list.count entries are lights) makes list.count a capacity: the prep
 	// (grb_light_prep[_shadowed]_counted) reads the live length under the same events; refresh() still sizes the frame
 	// from the capacity.
+	// With `by_id` the maps come by map id instead (grb_light_prep_shadow_ids): `shadow_ids` holds each input light's
+	// transform and id, and `map_table` (device, `map_table_size` entries) turns an id into this rank's map.
 	// Row-sharded frames whose list comes from one rank (scene_viewer.cpp, grbh_viewer_set_light_source_rank):
-	// `exchange` runs on the pass's stream after `ready` and may replace the list and count the prep reads with this
-	// frame's received copy; `after_prep` runs right behind the prep, before `consumed` and the cluster kernels.
+	// `exchange` runs on the pass's stream after `ready` and may replace the list, count and shadow ids the prep reads
+	// with this frame's received copy; `after_prep` runs right behind the prep, before `consumed` and the cluster kernels.
 	struct DeviceLightSource
 	{
 		GrbLightList list = {};
 		GrbLightShadowList shadows = {};
+		bool by_id = false;
+		GrbLightShadowIdList shadow_ids = {};
+		const void *const *map_table = nullptr;
+		int32_t map_table_size = 0;
 		const int32_t *input_count = nullptr;
-		std::function<void(Vulkan::CommandBuffer &, GrbLightList &, const int32_t *&)> exchange;
+		std::function<void(Vulkan::CommandBuffer &, GrbLightList &, const int32_t *&, GrbLightShadowIdList &)> exchange;
 		std::function<void(Vulkan::CommandBuffer &)> after_prep;
 		void *ready = nullptr, *consumed = nullptr;
 		void *scratch = nullptr; // grb_light_prep_scratch_bytes(list.count) or more

@@ -148,6 +148,27 @@ struct GrbhViewer
 	// its end, the flag words and counter of the source's push; allocated on the first such frame
 	void *light_slot = nullptr;
 	uint32_t light_slot_epoch = 0;
+	// this rank's shadow map table for device lights whose maps come by id (grbh_viewer_set_light_shadow_map_table): the
+	// caller's pointers, uploaded into the device table (GRBH_MAX_DEVICE_LIGHTS entries) on the clustering pass's stream
+	// by the first frame after a change, and the map events that go with the table
+	bool has_shadow_table = false, shadow_table_changed = false;
+	std::vector<const void *> shadow_table;
+	void *shadow_table_device = nullptr;
+	cudaEvent_t table_maps_ready = nullptr, table_maps_consumed = nullptr;
+	void upload_shadow_table(Vulkan::CommandBuffer &cmd)
+	{
+		if (!shadow_table_changed)
+			return;
+		// from pageable memory: the driver stages the bytes before the call returns (it may wait for the stream first; a
+		// table changes rarely), and the copy follows every earlier frame's prep on this stream, so frames already
+		// recorded keep the table they were recorded with
+		if (!shadow_table.empty() &&
+		    !Vulkan::cuda_ok(cudaMemcpyAsync(shadow_table_device, shadow_table.data(), sizeof(void *) * shadow_table.size(), cudaMemcpyHostToDevice,
+		                                     reinterpret_cast<cudaStream_t>(cmd.get_stream())),
+		                     "shadow map table upload"))
+			throw std::runtime_error("clustering: the upload of the shadow map table failed");
+		shadow_table_changed = false;
+	}
 	std::vector<mat_affine> scene_decals;
 
 	mat4 projection = mat4(1.0f), view = mat4(1.0f);
@@ -242,7 +263,7 @@ struct GrbhViewer
 	void set_output_ring(const GrbImage *images, int32_t count);
 	bool fed_from_source() const { return bands.size() > 1 && gbuffer_source >= 0; }
 	bool lights_from_source() const { return bands.size() > 1 && light_source >= 0; }
-	void exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count);
+	void exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count, GrbLightShadowIdList &ids);
 
 	// the G-buffer planes of the attachments (grb_gbuffer_copy_rows order), the G-buffer ones and / or motion vectors
 	GrbGBufferPlanes attachment_planes(bool gbuffer_planes, bool mv)
@@ -371,16 +392,18 @@ void GrbhViewer::bake_render_graph()
 	else
 		cluster.set_lit_pixel_rows(0, 0, 0);
 	cluster.set_lit_tile_ranges(striped() ? stripe_plan().tile_rows : std::vector<GrbRows>{});
-	if (lights_from_source())
-	{
-		device_lights.exchange = [this](Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count) { exchange_lights(cmd, list, count); };
-		device_lights.after_prep = [this](Vulkan::CommandBuffer &cmd) { light_handover.credit(cmd, rank); };
-	}
+	if (lights_from_source() || config.clustered_lights_shadows)
+		device_lights.exchange = [this](Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count, GrbLightShadowIdList &ids) {
+			upload_shadow_table(cmd);
+			if (lights_from_source())
+				exchange_lights(cmd, list, count, ids);
+		};
 	else
-	{
 		device_lights.exchange = nullptr;
+	if (lights_from_source())
+		device_lights.after_prep = [this](Vulkan::CommandBuffer &cmd) { light_handover.credit(cmd, rank); };
+	else
 		device_lights.after_prep = nullptr;
-	}
 	cluster.add_render_passes(graph);
 	lighting.cluster = &cluster;
 	context.set_lighting_parameters(&lighting);
@@ -881,14 +904,24 @@ void GrbhViewer::feed_from_source(Vulkan::CommandBuffer &cmd)
 // list's live entries into every rank's slot, then preps its own list; every other rank preps its slot (the list and
 // count returned here) and raises its credit behind the prep (`after_prep`).  Without peer memory: S fills its own
 // slot with the same kernel and a broadcast from S carries the whole slot into every rank's, in stream order with the
-// prep that reads it.
-void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count)
+// prep that reads it.  A shadowed viewer's slot also holds each live light's shadow transform and map id (the shadowed
+// slot of grb_light_shadow_slot_layout); every rank resolves the ids through its own map table.
+void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list, const int32_t *&count, GrbLightShadowIdList &ids)
 {
 	const unsigned S = (unsigned)light_source;
+	const bool shadowed = config.clustered_lights_shadows != 0;
 	void *handle = cmd.get_stream_handle();
 	uint64_t bytes = 0;
-	if (!cmd.check(grb_light_slot_layout(nullptr, nullptr, nullptr, &bytes), "grb_light_slot_layout"))
+	if (shadowed ? !cmd.check(grb_light_shadow_slot_layout(nullptr, nullptr, nullptr, &bytes), "grb_light_shadow_slot_layout")
+	             : !cmd.check(grb_light_slot_layout(nullptr, nullptr, nullptr, &bytes), "grb_light_slot_layout"))
 		return;
+	// S's push of its list (and shadow ids) into `slots`
+	auto push = [&](void *const *slots, uint32_t *const *flags, int32_t peers, int32_t index, uint32_t epoch, uint32_t *counter) {
+		if (shadowed)
+			cmd.check(grb_light_list_shadowed_to_peers(&list, &ids, count, slots, flags, peers, index, epoch, counter, handle), "grb_light_list_shadowed_to_peers");
+		else
+			cmd.check(grb_light_list_to_peers(&list, count, slots, flags, peers, index, epoch, counter, handle), "grb_light_list_to_peers");
+	};
 	RenderGraphCollectives *coll = graph.get_collectives();
 	void *received = nullptr;
 	if (light_handover.begin(cmd, *coll, (size_t)bytes, S, rank))
@@ -896,8 +929,7 @@ void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list,
 		const RenderGraphCollectives::PeerSlot &slot = light_handover.slot;
 		if (rank == S)
 		{
-			cmd.check(grb_light_list_to_peers(&list, count, slot.images, slot.flags, (int32_t)slot.count, (int32_t)S, slot.epoch, slot.counter, handle),
-			          "grb_light_list_to_peers");
+			push(slot.images, slot.flags, (int32_t)slot.count, (int32_t)S, slot.epoch, slot.counter);
 			return;
 		}
 		received = slot.images[rank];
@@ -920,7 +952,7 @@ void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list,
 		{
 			void *slots[1] = { light_slot };
 			uint32_t *flags[1] = { reinterpret_cast<uint32_t *>(static_cast<uint8_t *>(light_slot) + bytes) };
-			cmd.check(grb_light_list_to_peers(&list, count, slots, flags, 1, 0, ++light_slot_epoch, flags[0] + 8, handle), "grb_light_list_to_peers");
+			push(slots, flags, 1, 0, ++light_slot_epoch, flags[0] + 8);
 		}
 		if (!coll->broadcast_bytes(cmd.get_stream(), light_slot, (size_t)bytes, S))
 			throw std::runtime_error("clustering: the broadcast of the light list from the source rank failed");
@@ -937,6 +969,15 @@ void GrbhViewer::exchange_lights(Vulkan::CommandBuffer &cmd, GrbLightList &list,
 	slot_list.cutoff_range = list.cutoff_range;
 	list = slot_list;
 	count = slot_count;
+	if (shadowed)
+	{
+		float *transforms = nullptr;
+		int32_t *map_ids = nullptr;
+		if (!cmd.check(grb_light_shadow_slot_layout(received, &transforms, &map_ids, &bytes), "grb_light_shadow_slot_layout"))
+			return;
+		ids.transforms = transforms;
+		ids.map_ids = map_ids;
+	}
 }
 
 cudaStream_t GrbhViewer::enqueue_readback(uint32_t *dst, GrbRows &r)
@@ -1138,6 +1179,8 @@ extern "C" void grbh_viewer_destroy(GrbhViewer *viewer)
 		cudaFree(viewer->light_scratch);
 	if (viewer->light_slot)
 		cudaFree(viewer->light_slot);
+	if (viewer->shadow_table_device)
+		cudaFree(viewer->shadow_table_device);
 	if (viewer->device)
 		Granite::release_smaa_lookup_textures(*viewer->device); // device images: must go before the device does
 	delete viewer;
@@ -1178,6 +1221,8 @@ extern "C" int32_t grbh_viewer_set_lights(GrbhViewer *v, const GrbhLights *l)
 	v->cluster.set_device_lights(nullptr);
 	v->device_prep_rendered = false;
 	v->device_lights.shadows = {};
+	v->device_lights.by_id = false;
+	v->device_lights.shadow_ids = {};
 	v->device_lights.input_count = nullptr;
 	v->shadow_map_events.ready = v->shadow_map_events.consumed = nullptr;
 	v->light_storage.clear();
@@ -1283,6 +1328,8 @@ int32_t bind_device_lights(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhD
 	d.list.cutoff_range = l->cutoff_range;
 	d.shadows.transforms = sh ? sh->transforms : nullptr;
 	d.shadows.maps = sh ? reinterpret_cast<const void *const *>(sh->maps) : nullptr;
+	d.by_id = false;
+	d.shadow_ids = {};
 	d.input_count = nullptr; // a new list: every entry is live until grbh_viewer_set_light_count_device
 	d.ready = l->ready;
 	d.consumed = l->consumed;
@@ -1337,10 +1384,104 @@ extern "C" int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *v, const G
 		return fail(fn + "the viewer was created without clustered_lights_shadows (grbh_viewer_set_lights_device)");
 	if (l->count > 0 && (!shadows->transforms || !shadows->maps))
 		return fail(fn + "null shadow transforms or shadow maps table");
+	if (v->light_source >= 0)
+	{
+		const std::string receiver = not_light_source(v);
+		return fail(fn + (receiver.empty() ? "the light source rank binds shadowed device lights by map id, whose maps every rank resolves in its own "
+		                                     "table (grbh_viewer_set_lights_device_shadow_ids)"
+		                                   : receiver));
+	}
 	if (!v->device)
 		return fail(fn + "host-only viewer (no CUDA device)");
 	GRBH_TRY
 	return bind_device_lights(v, l, shadows, fn);
+	GRBH_CATCH
+}
+
+namespace
+{
+// the bound device list's shadows come by map id, through this rank's table and under the table's map events
+void bind_shadow_ids(GrbhViewer *v, const GrbhDeviceLightShadowIds *ids)
+{
+	auto &d = v->device_lights;
+	d.by_id = true;
+	d.shadow_ids.transforms = ids ? ids->transforms : nullptr;
+	d.shadow_ids.map_ids = ids ? ids->map_ids : nullptr;
+	v->shadow_map_events.ready = v->table_maps_ready;
+	v->shadow_map_events.consumed = v->table_maps_consumed;
+}
+} // namespace
+
+extern "C" int32_t grbh_viewer_set_light_shadow_map_table(GrbhViewer *v, const void *const *maps, int32_t count, void *maps_ready, void *maps_consumed)
+{
+	const std::string fn = "grbh_viewer_set_light_shadow_map_table: ";
+	if (!v)
+		return fail(fn + "null viewer");
+	if (count < 0 || count > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(fn + "count " + std::to_string(count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (count > 0 && !maps)
+		return fail(fn + "null map array with count > 0");
+	if (!v->config.clustered_lights_shadows)
+		return fail(fn + "the viewer was created without clustered_lights_shadows");
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	GRBH_TRY
+	cudaSetDevice(v->device->get_device_index());
+	for (int32_t i = 0; i < count; i++)
+		if (maps[i] && !is_viewer_device_memory(v, fn, ("map " + std::to_string(i)).c_str(), maps[i], 1))
+			return -1;
+	if (!v->shadow_table_device)
+	{
+		void *p = nullptr;
+		if (!Vulkan::cuda_ok(cudaMalloc(&p, sizeof(void *) * GRBH_MAX_DEVICE_LIGHTS), "cudaMalloc(shadow map table)"))
+			return fail(fn + "cudaMalloc of the device table failed");
+		v->shadow_table_device = p;
+	}
+	v->shadow_table.assign(maps, maps + count);
+	v->shadow_table_changed = true;
+	v->has_shadow_table = true;
+	v->table_maps_ready = static_cast<cudaEvent_t>(maps_ready);
+	v->table_maps_consumed = static_cast<cudaEvent_t>(maps_consumed);
+	auto &d = v->device_lights;
+	d.map_table = static_cast<const void *const *>(v->shadow_table_device);
+	d.map_table_size = count;
+	if (d.by_id && v->cluster.has_device_lights())
+	{
+		v->shadow_map_events.ready = v->table_maps_ready;
+		v->shadow_map_events.consumed = v->table_maps_consumed;
+	}
+	return 0;
+	GRBH_CATCH
+}
+
+extern "C" int32_t grbh_viewer_set_lights_device_shadow_ids(GrbhViewer *v, const GrbhDeviceLights *l, const GrbhDeviceLightShadowIds *ids)
+{
+	const std::string fn = "grbh_viewer_set_lights_device_shadow_ids: ";
+	if (!v || !l || !ids)
+		return fail(fn + "null viewer, light list or shadow id list");
+	if (l->count < 0 || l->count > GRBH_MAX_DEVICE_LIGHTS)
+		return fail(fn + "count " + std::to_string(l->count) + " is outside 0.." + std::to_string(GRBH_MAX_DEVICE_LIGHTS));
+	if (!v->config.clustered_lights_shadows)
+		return fail(fn + "the viewer was created without clustered_lights_shadows (grbh_viewer_set_lights_device)");
+	if (l->count > 0 && (!ids->transforms || !ids->map_ids))
+		return fail(fn + "null shadow transforms or map ids");
+	const std::string receiver = not_light_source(v);
+	if (!receiver.empty())
+		return fail(fn + receiver);
+	if (!v->device)
+		return fail(fn + "host-only viewer (no CUDA device)");
+	if (!v->has_shadow_table)
+		return fail(fn + "no shadow map table is set on this rank (grbh_viewer_set_light_shadow_map_table first)");
+	GRBH_TRY
+	cudaSetDevice(v->device->get_device_index());
+	if (l->count > 0 && (!is_viewer_device_memory(v, fn, "shadow transforms", ids->transforms, 64 * (size_t)l->count) ||
+	                     !is_viewer_device_memory(v, fn, "map ids", ids->map_ids, 4 * (size_t)l->count)))
+		return -1;
+	const int32_t rc = bind_device_lights(v, l, nullptr, fn);
+	if (rc != 0)
+		return rc;
+	bind_shadow_ids(v, ids);
+	return 0;
 	GRBH_CATCH
 }
 
@@ -1392,6 +1533,9 @@ extern "C" int32_t grbh_viewer_set_lights_device_from_source(GrbhViewer *v, int3
 	if (rc != 0)
 		return rc;
 	v->device_lights.list.count = capacity;
+	// a shadowed viewer's slot holds the shadow transforms and map ids too: resolved through this rank's table
+	if (v->config.clustered_lights_shadows)
+		bind_shadow_ids(v, nullptr);
 	return 0;
 	GRBH_CATCH
 }
@@ -1567,8 +1711,9 @@ extern "C" int32_t grbh_viewer_set_light_source_rank(GrbhViewer *v, int32_t rank
 	const std::string fn = "grbh_viewer_set_light_source_rank: ";
 	if (!v)
 		return fail(fn + "null viewer");
-	if (rank >= 0 && v->config.clustered_lights_shadows)
-		return fail(fn + "not with clustered_lights_shadows (a light's shadow map pointer is valid on its own rank only)");
+	if (rank >= 0 && v->config.clustered_lights_shadows && !v->has_shadow_table)
+		return fail(fn + "not with clustered_lights_shadows (a light's shadow map pointer is valid on its own rank only) unless a shadow map table "
+		                 "is set (grbh_viewer_set_light_shadow_map_table)");
 	const int32_t count = std::max((int32_t)v->bands.size(), 1); // an unsharded viewer is one band
 	if (rank < -1 || rank >= count)
 		return fail(fn + "rank must be -1 (off) or within [0, " + std::to_string(count) + ") (the bands of the last grbh_viewer_set_row_shards)");

@@ -42,6 +42,10 @@ class GrbhDeviceLightShadows(C.Structure):
     _fields_ = [("transforms", C.c_void_p), ("maps", C.c_void_p), ("maps_ready", C.c_void_p), ("maps_consumed", C.c_void_p)]
 
 
+class GrbhDeviceLightShadowIds(C.Structure):
+    _fields_ = [("transforms", C.c_void_p), ("map_ids", C.c_void_p)]
+
+
 MAX_DEVICE_LIGHTS = 65536
 
 
@@ -78,6 +82,8 @@ def lib() -> C.CDLL:
         _lib.grbh_viewer_acquire_output.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         _lib.grbh_viewer_set_light_count_device.argtypes = [C.c_void_p, C.c_void_p]
         _lib.grbh_viewer_set_lights_device_from_source.argtypes = [C.c_void_p, C.c_int32, C.c_float]
+        _lib.grbh_viewer_set_light_shadow_map_table.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        _lib.grbh_viewer_set_lights_device_shadow_ids.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _lib
 
 
@@ -415,7 +421,7 @@ class Viewer:
         _check(lib().grbh_viewer_set_lights(self._h, C.byref(l)), "grbh_viewer_set_lights")
 
     def set_lights_device(self, color, position, is_point, rotation, inner_cone, outer_cone, cutoff=1e10, ready=None, consumed=None,
-                          shadow_transforms=None, shadow_maps=None, maps_ready=None, maps_consumed=None, count=None):
+                          shadow_transforms=None, shadow_maps=None, maps_ready=None, maps_consumed=None, count=None, shadow_map_ids=None):
         """Binds a light list in device memory (grbh_viewer_set_lights_device) from the next frame until the next
         set_lights[_device] call: torch CUDA tensors on the viewer's device, contiguous, in synth.Lights' shapes --
         color and position (N, 3) float32, is_point (N,) bool or uint8, rotation (N, 3, 3) float32 column-major,
@@ -430,20 +436,33 @@ class Viewer:
         ready / consumed.  maps_ready: a torch.cuda.Event the lighting pass waits on before it samples the maps;
         maps_consumed: one the viewer records behind the lighting pass's last read of them.
 
+        shadow_map_ids (N,) int32 in place of shadow_maps names each light's map by its index in this rank's table
+        (set_light_shadow_map_table, which also takes the map events); an id outside the table means no shadow
+        (grbh_viewer_set_lights_device_shadow_ids).  This is the form a light source rank binds with
+        (set_light_source_rank): an id means the same map on every rank, a pointer does not.
+
         count: a torch CUDA int32 tensor of one element, on the viewer's device, holding the list's live length
         (grbh_viewer_set_light_count_device).  N is then a capacity: each frame reads the count under ready / consumed
         and renders the first min(max(count, 0), N) lights, so a GPU pass that spawns, kills or compacts lights can
         rewrite it between frames without a host sync.  Entries past it are never read.  Without it all N are lights."""
         import torch
 
-        shadowed = shadow_transforms is not None or shadow_maps is not None
+        if shadow_maps is not None and shadow_map_ids is not None:
+            raise ValueError("set_lights_device: shadow_maps and shadow_map_ids together; a light's map is named by pointer or by id")
+        by_id = shadow_map_ids is not None
+        if by_id and (maps_ready is not None or maps_consumed is not None):
+            raise ValueError("set_lights_device: with shadow_map_ids the map events go with the table (set_light_shadow_map_table)")
+        shadowed = shadow_transforms is not None or shadow_maps is not None or by_id
         n = int(color.shape[0]) if isinstance(color, torch.Tensor) and color.dim() == 2 else -1
         want = {"color": (color, [(n, 3)], (torch.float32,)), "position": (position, [(n, 3)], (torch.float32,)),
                 "is_point": (is_point, [(n,)], (torch.bool, torch.uint8)), "rotation": (rotation, [(n, 3, 3)], (torch.float32,)),
                 "inner_cone": (inner_cone, [(n,)], (torch.float32,)), "outer_cone": (outer_cone, [(n,)], (torch.float32,))}
         if shadowed:
             want["shadow_transforms"] = (shadow_transforms, [(n, 16), (n, 4, 4)], (torch.float32,))
-            want["shadow_maps"] = (shadow_maps, [(n,)], (torch.int64,))
+            if by_id:
+                want["shadow_map_ids"] = (shadow_map_ids, [(n,)], (torch.int32,))
+            else:
+                want["shadow_maps"] = (shadow_maps, [(n,)], (torch.int64,))
         for name, (t, shapes, dtypes) in want.items():
             if not isinstance(t, torch.Tensor) or not t.is_cuda:
                 raise ValueError(f"set_lights_device: {name} must be a torch CUDA tensor")
@@ -470,7 +489,11 @@ class Viewer:
 
         l = GrbhDeviceLights(n, color.data_ptr(), position.data_ptr(), is_point.data_ptr(), rotation.data_ptr(), inner_cone.data_ptr(),
                              outer_cone.data_ptr(), cutoff, ev(ready), ev(consumed))
-        if shadowed:
+        if by_id:
+            ids = GrbhDeviceLightShadowIds(shadow_transforms.data_ptr(), shadow_map_ids.data_ptr())
+            _check(lib().grbh_viewer_set_lights_device_shadow_ids(self._h, C.byref(l), C.byref(ids)), "grbh_viewer_set_lights_device_shadow_ids")
+            self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone, shadow_transforms, shadow_map_ids)
+        elif shadowed:
             sh = GrbhDeviceLightShadows(shadow_transforms.data_ptr(), shadow_maps.data_ptr(), ev(maps_ready), ev(maps_consumed))
             _check(lib().grbh_viewer_set_lights_device_shadowed(self._h, C.byref(l), C.byref(sh)), "grbh_viewer_set_lights_device_shadowed")
             self._device_lights = (color, position, is_point, rotation, inner_cone, outer_cone, shadow_transforms, shadow_maps)
@@ -505,12 +528,28 @@ class Viewer:
         sets the same value, before bake; not with pipelined_io (grbh_viewer_set_gbuffer_source_rank)."""
         _check(lib().grbh_viewer_set_gbuffer_source_rank(self._h, int(rank)), "grbh_viewer_set_gbuffer_source_rank")
 
+    def set_light_shadow_map_table(self, pointers, maps_ready=None, maps_consumed=None):
+        """This rank's shadow map table for device lights whose maps come by id (set_lights_device(shadow_map_ids=)):
+        `pointers` are this rank's map data_ptr()s (ints, 0 = no shadow), copied into a table the viewer owns; a
+        replaced table takes effect from the next frame.  maps_ready / maps_consumed: torch.cuda.Events the lighting
+        pass waits on before it samples the maps and records behind its last read
+        (grbh_viewer_set_light_shadow_map_table)."""
+        ptrs = [int(p) for p in pointers]
+        arr = (C.c_void_p * max(len(ptrs), 1))(*[p or None for p in ptrs])
+        for e in (maps_ready, maps_consumed):
+            if e is not None and not e.cuda_event:
+                e.record()  # torch creates the CUDA event on its first record
+        _check(lib().grbh_viewer_set_light_shadow_map_table(self._h, arr, len(ptrs), None if maps_ready is None else maps_ready.cuda_event,
+                                                            None if maps_consumed is None else maps_consumed.cuda_event),
+               "grbh_viewer_set_light_shadow_map_table")
+
     def set_light_source_rank(self, rank):
         """Row-sharded frames whose device light list comes from `rank` (-1: off): that rank binds its list (and count)
         with set_lights_device, every other rank calls set_lights_device_from_source with the same capacity and cutoff
         between the same two frames, and each frame pushes the list's live entries and count from that rank into every
-        other rank's clustering pass.  Every rank sets the same value, before bake; not with light_shadows
-        (grbh_viewer_set_light_source_rank)."""
+        other rank's clustering pass.  Every rank sets the same value, before bake.  With light_shadows every rank
+        first sets its own map table (set_light_shadow_map_table) and the source rank binds with shadow_map_ids: the
+        transforms and ids travel with the list (grbh_viewer_set_light_source_rank)."""
         _check(lib().grbh_viewer_set_light_source_rank(self._h, int(rank)), "grbh_viewer_set_light_source_rank")
 
     def set_lights_device_from_source(self, capacity, cutoff=1e10):

@@ -235,6 +235,26 @@ int32_t grb_light_prep_shadowed_counted(const GrbLightList *lights, const int32_
                                         const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask, uint32_t *z_ranges,
                                         float *shadow_transforms_out, const void **shadow_maps_out, int32_t *device_count, void *scratch,
                                         uint64_t scratch_bytes, void *stream);
+/* The shadows of a GrbLightList by map id, in the same input order: each light's transform and the index of its map in
+ * a table of map pointers that every rank holds for itself.  An id travels between ranks where a pointer cannot. */
+typedef struct GrbLightShadowIdList
+{
+	const float *transforms; /* count x 16, column-major, device */
+	const int32_t *map_ids;  /* count map ids (4-byte aligned), device */
+} GrbLightShadowIdList;
+/* grb_light_prep_shadowed[_counted] with the maps named by id: slot s < count gets the transform of the input light
+ * packed into slot s and map_table[id] of its id when 0 <= id < table_size, a null map otherwise (an id written on the
+ * device cannot be refused, so one out of range means no shadow); slots [count, slots) a zero matrix and a null map.
+ * map_table: table_size device pointers (8-byte aligned array), device, null entries allowed.  input_count: as for the
+ * _counted forms, NULL = every entry is live; entries at or past live are never read, not their ids nor their
+ * transforms.  Same three launches; the other outputs are grb_light_prep's bytes.  GRB_ERR_INVALID_ARGUMENT: what
+ * grb_light_prep_shadowed refuses, null ids or transforms with count > 0, a table_size outside 0..GRB_MAX_LIGHT_LIST,
+ * a null table with table_size > 0, a table that is not 8-byte aligned, ids that are not 4-byte aligned, a misaligned
+ * input_count. */
+int32_t grb_light_prep_shadow_ids(const GrbLightList *lights, const int32_t *input_count, const GrbLightShadowIdList *ids, const void *const *map_table,
+                                  int32_t table_size, const GrbLightPrepView *view, GrbPositionalLight *records, float *model, uint32_t *type_mask,
+                                  uint32_t *z_ranges, float *shadow_transforms_out, const void **shadow_maps_out, int32_t *device_count, void *scratch,
+                                  uint64_t scratch_bytes, void *stream);
 /* The largest light list the prep takes (GRBH_MAX_DEVICE_LIGHTS of the host API). */
 #define GRB_MAX_LIGHT_LIST 65536
 /* The light slot of a row-sharded frame's light channel: a GrbLightList of GRB_MAX_LIGHT_LIST entries plus the count
@@ -258,6 +278,19 @@ int32_t grb_light_slot_layout(void *slot, GrbLightList *out, int32_t **count_out
  * written).  No reference equivalent (the reference never splits a frame). */
 int32_t grb_light_list_to_peers(const GrbLightList *lights, const int32_t *input_count, void *const *peer_slots, uint32_t *const *peer_flags,
                                 int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter, void *stream);
+/* The shadow part of a shadowed light slot: it starts at the end of the light slot (grb_light_slot_layout's size) and
+ * holds GRB_MAX_LIGHT_LIST shadow transforms (64 bytes each) and then as many map ids (GrbLightShadowIdList order),
+ * each array from a multiple of 256 bytes.  *bytes receives the size of the whole shadowed slot, light slot included
+ * (about 9 MB).  slot (16-byte aligned) may be NULL to query the size only; transforms and map_ids (may be NULL) then
+ * receive NULL.  GRB_ERR_INVALID_ARGUMENT: a null `bytes`, a slot that is not 16-byte aligned. */
+int32_t grb_light_shadow_slot_layout(void *slot, float **transforms, int32_t **map_ids, uint64_t *bytes);
+/* grb_light_list_to_peers for a shadowed list: in the same one launch it also stores bytes [0, live x element size) of
+ * ids->transforms and ids->map_ids into the shadow part of every slot (grb_light_shadow_slot_layout), then publishes
+ * the same way.  No entry at or past live is read.  GRB_ERR_INVALID_ARGUMENT: what grb_light_list_to_peers refuses, null
+ * ids, null transforms or map ids with count > 0 (checked before any CUDA call; nothing is written). */
+int32_t grb_light_list_shadowed_to_peers(const GrbLightList *lights, const GrbLightShadowIdList *ids, const int32_t *input_count, void *const *peer_slots,
+                                         uint32_t *const *peer_flags, int32_t peer_count, int32_t flag_index, uint32_t epoch, uint32_t *scratch_counter,
+                                         void *stream);
 
 /* Volumetric-decal binning over the clusterer's tile grid: LightClusterer::update_bindless_mask_buffer_decal_gpu
  * (clusterer.cpp:1391-1461) + clusterer_bindless_binning_decal.comp.  mvps: num_decals x mat4 (column-major, device) =

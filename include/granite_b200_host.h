@@ -114,6 +114,15 @@ typedef struct GrbhDeviceLightShadows
 	void *maps_consumed;     /* cudaEvent_t or NULL: recorded on the lighting pass's stream behind its last read of the maps */
 } GrbhDeviceLightShadows;
 
+/* The shadows of a device light list by map id (grbh_viewer_set_lights_device_shadow_ids), in the lights' input order:
+ * each light's transform, as in GrbhDeviceLightShadows, and the index of its map in this rank's shadow map table
+ * (grbh_viewer_set_light_shadow_map_table).  An id outside 0..table count - 1 means no shadow. */
+typedef struct GrbhDeviceLightShadowIds
+{
+	const float *transforms; /* device, count x 16, column-major */
+	const int32_t *map_ids;  /* device, count map ids */
+} GrbhDeviceLightShadowIds;
+
 /* Host-memory G-buffer of the full frame (pinned memory makes the uploads asynchronous).
  * Only the rows this rank needs (its band + halo) are copied.  mv may be NULL without TAA. */
 typedef struct GrbhHostGBuffer
@@ -166,6 +175,25 @@ int32_t grbh_viewer_set_lights_device(GrbhViewer *viewer, const GrbhDeviceLights
  * a viewer created without clustered_lights_shadows, null tables with count > 0, a host-only viewer, arrays or tables
  * that are not device memory of the viewer's device. */
 int32_t grbh_viewer_set_lights_device_shadowed(GrbhViewer *viewer, const GrbhDeviceLights *lights, const GrbhDeviceLightShadows *shadows);
+/* This rank's shadow map table for shadowed device lights whose maps come by id: maps is a HOST array of `count` device
+ * map pointers of this rank (null = no shadow; maps as grbh_viewer_set_light_shadow_maps takes them), copied into a
+ * device table the viewer owns.  A replaced table takes effect from the next frame: the upload is ordered on the
+ * clustering pass's stream, so frames already recorded keep the table they were recorded with.  maps_ready /
+ * maps_consumed (cudaEvent_t or NULL) go to the lighting pass as for grbh_viewer_set_lights_device_shadowed: it waits on
+ * the first before it samples the maps and records the second behind its last read.  The caller owns the maps on every
+ * rank (renders them there, or copies static maps there once); no texel crosses between ranks.  Refused: a null
+ * viewer, a count outside 0..GRBH_MAX_DEVICE_LIGHTS, a null array with count > 0, a viewer created without
+ * clustered_lights_shadows, a host-only viewer, a non-null entry that is not device memory of the viewer's device. */
+int32_t grbh_viewer_set_light_shadow_map_table(GrbhViewer *viewer, const void *const *maps, int32_t count, void *maps_ready, void *maps_consumed);
+/* grbh_viewer_set_lights_device_shadowed with each light's map named by id: the clustering pass moves each kept light's
+ * transform into cluster order and resolves its id through this rank's table (an id outside the table: no shadow), so
+ * frames equal those of host lights given table[id].  On one GPU, on each rank and on the light source rank of
+ * grbh_viewer_set_light_source_rank, whose push carries the transforms and ids to every other rank.
+ * grbh_viewer_set_light_count_device applies to it.  Refused: a null argument, a count outside
+ * 0..GRBH_MAX_DEVICE_LIGHTS, a viewer created without clustered_lights_shadows, null arrays with count > 0, a rank that
+ * receives its lights from the light source rank, a host-only viewer, no table set on this rank, arrays that are not
+ * device memory of the viewer's device. */
+int32_t grbh_viewer_set_lights_device_shadow_ids(GrbhViewer *viewer, const GrbhDeviceLights *lights, const GrbhDeviceLightShadowIds *ids);
 /* Gives the device light list bound now (shadowed or not) a length that lives on the device: its `count` becomes the
  * capacity, and every frame's clustering pass reads *count under the lights' ready / consumed events, so a GPU pass may
  * rewrite it between frames with no host read.  Entries [0, live) are the lights, live = min(max(*count, 0), capacity)
@@ -259,14 +287,20 @@ int32_t grbh_viewer_set_gbuffer_source_rank(GrbhViewer *viewer, int32_t rank);
  * count (DESIGN.md section 5, "Lights from device memory").
  * Collective contract: every rank sets the same value before bake.  Every binding on S (with or without a count) is
  * matched by a receiving binding of the same capacity and cutoff on every other rank, between the same two frames;
- * grbh_viewer_set_lights (host lights) is called on every rank or on none.  Refused: a viewer created with
- * clustered_lights_shadows (a light's shadow map pointer is only valid on its own rank), a rank out of range, a call
- * after bake. */
+ * grbh_viewer_set_lights (host lights) is called on every rank or on none.
+ * Shadowed viewers (clustered_lights_shadows): a map pointer is valid on its own rank only, so the maps go by id.  Every
+ * rank first sets its own shadow map table (grbh_viewer_set_light_shadow_map_table); S binds with
+ * grbh_viewer_set_lights_device_shadow_ids (grbh_viewer_set_lights_device_shadowed is refused there), and every other
+ * rank's receiving binding then preps the transforms and ids S pushed with the list, resolving each id through its own
+ * table, so grbh_viewer_get_light_shadow_prep returns this rank's pointers.  Collective contract, on top of the one
+ * above: every rank's table has the same count, and for each id every rank's map has the same texels.
+ * Refused: a shadowed viewer without a shadow map table, a rank out of range, a call after bake. */
 int32_t grbh_viewer_set_light_source_rank(GrbhViewer *viewer, int32_t rank);
 /* The receiving binding of a rank other than the light source rank: from the next frame, the clustering pass preps the
  * list the source rank pushed this frame, as a list of `capacity` entries with cutoff_range, so the frame is sized from
  * `capacity` exactly as on the source rank.  The pushed count is clamped to `capacity`.  grbh_viewer_get_light_prep
- * reads this rank's own prep.  Refused: a null viewer, a viewer with no light source rank, the light source rank itself,
+ * reads this rank's own prep.  On a shadowed viewer the prep also reads the slot's shadow transforms and map ids and
+ * resolves the ids through this rank's table.  Refused: a null viewer, a viewer with no light source rank, the light source rank itself,
  * a capacity outside 0..GRBH_MAX_DEVICE_LIGHTS, a host-only viewer. */
 int32_t grbh_viewer_set_lights_device_from_source(GrbhViewer *viewer, int32_t capacity, float cutoff_range);
 /* The row ranges of the render-size G-buffer this rank reads: its lighting rows (grbh_shard_plan*), or the upload list

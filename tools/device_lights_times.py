@@ -6,13 +6,18 @@ moved every frame by a small torch op on the device, by where the light prep run
 - "device lights": set_lights_device binds the tensors once; every frame's clustering pass culls, sorts and packs them
   on the GPU.
 
-    python tools/device_lights_times.py [--frames 100] [--shadows | --live-count]
-    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows | --live-count [--source-rank]]
+    python tools/device_lights_times.py [--frames 100] [--shadows [--map-ids] | --live-count]
+    torchrun --nproc-per-node=<GPUs> tools/device_lights_times.py [--frames 100] [--shadows [--map-ids] | [--shadows] --live-count [--source-rank]]
 
 --shadows: viewers created with clustered_lights_shadows, every light shadowed by one of 64 static synthetic cube maps
 (64 x 64 texels a face).  Host lights get the map pointers with set_lights every frame and the clusterer computes the
 shadow transforms; device lights bind the transforms (the reference's, computed once: a point light's depends only on
 its range) and the pointers with the lights, and the clustering pass moves them into cluster order.
+
+--shadows --map-ids: a third mode, "device lights by map id": the same lights and transforms bound with map ids into a
+table of the 64 maps (set_light_shadow_map_table, set_lights_device(shadow_map_ids=)), so the clustering pass resolves
+each kept light's id through the table.  Its "clustering-bindless" time against the pointer form's is what the id
+costs.
 
 --live-count: a particle-style list whose length is known only on the device.  16384 particle lights, each alive for a
 lifetime of its own in a cycle of its own, so that about half are alive and the set changes every frame.  Every frame a
@@ -35,6 +40,8 @@ the list from the rank that simulates it:
 - "viewer push": rank 0 updates, compacts and binds once; every other rank binds a receiving list once
   (set_light_source_rank(0), set_lights_device_from_source), and rank 0's clustering pass pushes the live entries and
   the count to the other ranks.
+With --shadows every particle is shadowed by one of the 64 static cube maps, named by map id: every rank sets its own
+table of its own copy of the maps, and the transforms and ids follow the compaction, the broadcast and the push.
 
 Two light lists: 4096 input lights (all in view), and 16384 input lights of which 4096 are kept.  Under torchrun, one
 rank per GPU, row-sharded frames with every rank binding its own copy of the lights; the sharded rate is that of the
@@ -87,12 +94,16 @@ def shadow_inputs(scene, lights):
     pointers = maps.data_ptr() + 2 * 6 * SHADOW_RES * SHADOW_RES * (np.arange(n, dtype=np.int64) % SHADOW_MAPS)
     host = viewer.Viewer(W, H, cuda_device=-1, light_shadows=True, shadow_resolution=SHADOW_RES)
     host.set_camera(scene.projection, scene.view)
-    host.set_lights(lights)
-    host.set_light_shadow_maps(list(range(1, n + 1)))
-    t, m = host.light_shadow_prep()
-    host.close()
     transforms = np.zeros((n, 16), np.float32)
-    transforms[m.astype(np.int64) - 1] = t
+    # in chunks the host prep keeps whole (4096 lights): a light it culls keeps a zero matrix, which no frame packs
+    for at in range(0, n, 4096):
+        k = min(4096, n - at)
+        host.set_lights(synth.Lights(*[a[at:at + k] for a in (lights.color, lights.position, lights.is_point, lights.rot, lights.inner_cone,
+                                                              lights.outer_cone)]))
+        host.set_light_shadow_maps(list(range(1, k + 1)))
+        t, m = host.light_shadow_prep()
+        transforms[at + m.astype(np.int64) - 1] = t
+    host.close()
     return maps, pointers, transforms
 
 
@@ -110,12 +121,15 @@ def particles():
     return lights, cycle, lifetime, offset
 
 
-def live_count_stepper(mode, lights, cycle, lifetime, offset, rank=0):
+def live_count_stepper(mode, lights, cycle, lifetime, offset, rank=0, shadows=None):
     """step(v, i) for one --live-count mode: the particle update, the compaction (or the parking) and the frame.  The
     --source-rank modes: "every rank updates" is "device count" on every rank; under "caller broadcast" and "viewer
-    push" only rank 0 updates."""
+    push" only rank 0 updates.  shadows: (transforms, map ids, table) of shadowed particles by map id, or None."""
     n = PARTICLES
     src = cases.to_device(lights)
+    if shadows is not None:
+        src["shadow_transforms"] = torch.from_numpy(shadows[0]).cuda()
+        src["shadow_map_ids"] = torch.from_numpy(shadows[1]).cuda()
     cycle_t, lifetime_t, offset_t = (torch.from_numpy(a).cuda() for a in (cycle, lifetime, offset))
     # the compacted list, one row more than the capacity: dead particles are scattered into the last row
     out = {k: torch.empty((n + 1, *t.shape[1:]), dtype=t.dtype, device="cuda") for k, t in src.items()}
@@ -131,6 +145,8 @@ def live_count_stepper(mode, lights, cycle, lifetime, offset, rank=0):
         if state["viewer"] is not v:
             state["viewer"] = v
             state["gbs"] = [v.device_gbuffer(*g) for g in state["dev"]]
+            if shadows is not None and mode != "viewer push":  # source_rank_viewer sets it before the source rank
+                v.set_light_shadow_map_table(shadows[2])
             if mode == "viewer push" and receiver:
                 v.set_lights_device_from_source(n)
             elif mode in ("device count", "every rank updates", "caller broadcast", "viewer push"):
@@ -172,8 +188,9 @@ def live_count_stepper(mode, lights, cycle, lifetime, offset, rank=0):
     return step, state
 
 
-def source_rank_viewer(scene, bands, **config):
-    """sharded.make_viewer's row-sharded viewer with light source rank 0, which must be set before bake (collective)."""
+def source_rank_viewer(scene, bands, table=None, **config):
+    """sharded.make_viewer's row-sharded viewer with light source rank 0, which must be set before bake (collective); a
+    shadowed viewer sets its map table first."""
     v = viewer.Viewer(W, H, cuda_device=torch.cuda.current_device(), **config)
     v.set_directional(scene.dir_color, scene.dir_direction)
     rank = torch.distributed.get_rank()
@@ -183,6 +200,8 @@ def source_rank_viewer(scene, bands, **config):
     torch.distributed.broadcast(uid, 0)
     v.init_collectives(uid.cpu().numpy().tobytes(), rank, torch.distributed.get_world_size())
     v.set_row_shards(bands, rank)
+    if table is not None:
+        v.set_light_shadow_map_table(table)
     v.set_light_source_rank(0)
     v.set_camera(scene.projection, scene.view)
     v.bake()
@@ -191,19 +210,25 @@ def source_rank_viewer(scene, bands, **config):
 
 def live_count_runs(args, scene, dev, bands, card, distributed, rank, world):
     lights, cycle, lifetime, offset = particles()
+    shadows, shadow_cfg = None, {}
+    if args.shadows:
+        maps, _, transforms = shadow_inputs(scene, lights)
+        shadows = (transforms, (np.arange(PARTICLES) % SHADOW_MAPS).astype(np.int32), map_table(maps))
+        shadow_cfg = dict(light_shadows=True, shadow_resolution=SHADOW_RES)
     closer = sharded.close_sharded if distributed else (lambda v: v.close())
     runs = []
     modes = ("every rank updates", "caller broadcast", "viewer push") if args.source_rank else ("device count", "count read back", "parked")
     for mode in modes:
         times = []
         for timestamps in (False, True):
-            step, state = live_count_stepper(mode, lights, cycle, lifetime, offset, rank)
+            step, state = live_count_stepper(mode, lights, cycle, lifetime, offset, rank, shadows)
             state["dev"] = dev
             stream = torch.cuda.Stream()
             if mode == "viewer push":
-                v = source_rank_viewer(scene, bands, stream=stream.cuda_stream, timestamps=timestamps)
+                v = source_rank_viewer(scene, bands, shadows[2] if shadows else None, stream=stream.cuda_stream, timestamps=timestamps, **shadow_cfg)
             else:
-                v = sharded.make_viewer(W, H, scene, synth.make_lights(0), scene.view, bands=bands, stream=stream.cuda_stream, timestamps=timestamps)
+                v = sharded.make_viewer(W, H, scene, synth.make_lights(0), scene.view, bands=bands, stream=stream.cuda_stream, timestamps=timestamps,
+                                        **shadow_cfg)
             times.append(timed(v, stream, args.frames, step))
             if timestamps:
                 t, c = v.collect_timings().get("clustering-bindless", (0.0, 0))
@@ -222,6 +247,11 @@ def live_count_runs(args, scene, dev, bands, card, distributed, rank, world):
             run["frames_per_s"] = round(args.frames / (ms * 1e-3), 2)
         runs.append(run)
     return runs
+
+
+def map_table(maps):
+    """The map pointers of the 64 cube maps of `maps`, in order: the table whose id k names map k."""
+    return [maps[k].data_ptr() for k in range(SHADOW_MAPS)]
 
 
 def timed(v, stream, frames, step):
@@ -250,9 +280,12 @@ def main():
     ap.add_argument("--shadows", action="store_true", help="shadowed lights with static synthetic maps")
     ap.add_argument("--live-count", action="store_true", help="a compacted particle list whose length is known only on the device")
     ap.add_argument("--source-rank", action="store_true", help="with --live-count under torchrun: hand the list over from rank 0")
+    ap.add_argument("--map-ids", action="store_true", help="with --shadows: also bind the shadowed lights by map id")
     args = ap.parse_args()
-    if args.shadows and args.live_count:
-        ap.error("--shadows and --live-count are separate workloads")
+    if args.shadows and args.live_count and not args.source_rank:
+        ap.error("--shadows with --live-count is the --source-rank workload (shadows by map id)")
+    if args.map_ids and not args.shadows:
+        ap.error("--map-ids is a form of --shadows")
     distributed = "RANK" in os.environ
     if args.source_rank and not (args.live_count and distributed):
         ap.error("--source-rank times the --live-count workload on row-sharded frames: run it with --live-count under torchrun")
@@ -270,7 +303,8 @@ def main():
               "frames_timed": args.frames, "fill_frames": FILL, "ranks": world, "gpu": card, "runs": []}
     if args.live_count:
         result["workload"] = (f"c3: 3840x2160, bloom + tonemap, device G-buffer every frame, {PARTICLES} particle lights of which about half "
-                              "are alive, compacted on the device every frame" + (", handed over from rank 0" if args.source_rank else ""))
+                              "are alive, compacted on the device every frame" + (", handed over from rank 0" if args.source_rank else "") +
+                              (f", every light shadowed by map id ({SHADOW_RES}^2 cube maps, static)" if args.shadows else ""))
         result["runs"] = live_count_runs(args, scene, dev, bands, card, distributed, rank, world)
         if rank == 0:
             print(json.dumps(result), flush=True)
@@ -284,7 +318,10 @@ def main():
         if args.shadows:
             maps, pointers, transforms = shadow_inputs(scene, lights)
             shadow_args = dict(shadow_transforms=torch.from_numpy(transforms).cuda(), shadow_maps=torch.from_numpy(pointers).cuda())
-        for mode in ("host lights", "device lights"):
+            id_args = dict(shadow_transforms=shadow_args["shadow_transforms"],
+                           shadow_map_ids=torch.from_numpy((np.arange(n) % SHADOW_MAPS).astype(np.int32)).cuda())
+        modes = ("host lights", "device lights") + (("device lights by map id",) if args.map_ids else ())
+        for mode in modes:
             def make(extra):
                 v = sharded.make_viewer(W, H, scene, lights, scene.view, bands=bands, **shadow_cfg, **extra)
                 if args.shadows:
@@ -302,6 +339,9 @@ def main():
                         state["gbs"] = [v.device_gbuffer(*g) for g in dev]
                         if mode == "device lights":
                             v.set_lights_device(**d, **(shadow_args if args.shadows else {}))
+                        elif mode == "device lights by map id":
+                            v.set_light_shadow_map_table(map_table(maps))
+                            v.set_lights_device(**d, **id_args)
                     d["position"].add_(phase)  # the lights' own per-frame update, on the device
                     if mode == "host lights":
                         v.set_lights(synth.Lights(lights.color, d["position"].cpu().numpy(), lights.is_point, lights.rot, lights.inner_cone,
